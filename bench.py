@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Headline benchmark: edges/s of one DynConv2d forward (dilated kNN graph + EdgeConv,
-B=16 N=4096 k=20 C=64 - BASELINE.json's metric shape) on N B200s.
+B=16 N=4096 k=20 C=64 - BASELINE.json's metric shape) on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over one batch of 16 synthetic clouds
 (1,310,720 edges).  Multi-GPU: the batch dimension is sharded, every rank owns its
@@ -20,11 +20,16 @@ thread count that is fastest on this box (the reference's N^2 elementwise passes
 memory bound: all 128 hardware threads are slower than 16-32).
 
 At N = 1 the line also carries `gpu_reference` (the reference's op sequence - oracle
-port - running as torch-eager CUDA kernels on the same B200, the comparison target of
+port - running as torch-eager CUDA kernels on the same GPU, the comparison target of
 north_star's ">= 10x the reference GPU path") and `sustained` (the same step looped
 for >= 2 s with clocks sampled).  At N > 1 `extra` carries the node-partitioned
 GENConv stack on the products-shaped graph (`sparse_halo`) and one data-parallel
 MRGCN-28 training step (`ddp_mrgcn`), each with its parity check (bench_multigpu.py).
+
+`--dump-outputs DIR` writes what the last timed step returned (the DynConv2d output y, float32, 16.8 MB) to
+DIR/y.npy; at N > 1 every rank writes its own shard as DIR/y_rank<r>.npy (a fixed sample of it where all shards
+together would exceed 64 MB); `--impl reference` ignores the option.  Inputs and parameters are seeded, so two builds run with the same arguments can be compared output for
+output.
 """
 import argparse
 import json
@@ -44,7 +49,7 @@ EDGES_PER_STEP = B * N * K_NEIGH
 ALGO_BYTES_PER_EDGE = (C + C) * 4.0 / K_NEIGH            # 25.6 B
 # fp32 work per edge: distance contraction 2*N*C/k + factorised MLP 2*2C*C/k (SURVEY.md 8d)
 FLOPS_PER_EDGE = 2.0 * N * C / K_NEIGH + 2.0 * 2 * C * C / K_NEIGH
-N_ROTATE = 8                                             # 8 x 16.8 MB inputs = 134 MB > 126 MB L2
+N_ROTATE = 8                                             # 8 x 16.8 MB inputs = 134 MB > 50 MB L2
 WORKLOAD = "DynConv2d(64,64,k=20,d=1,edge,relu,batch).eval() fwd, x=randn(16,64,4096,1)"
 
 
@@ -57,6 +62,8 @@ def parse():
     ap.add_argument("--cpu-seconds", type=float, default=12.0, help="budget of the cpu_baseline leg")
     ap.add_argument("--sustained-seconds", type=float, default=2.0, help="length of the sustained loop (N=1)")
     ap.add_argument("--no-extra", action="store_true", help="skip the multi-GPU extra blocks (N>1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's output to DIR/y.npy (float32)")
     return ap.parse_args()
 
 
@@ -116,13 +123,19 @@ def thread_candidates():
 
 
 def peaks():
+    """(HBM GB/s, its source, max SM MHz, bf16 TFLOP/s, its source).  Figures missing from MEASURED_PEAKS.json come
+    from NVIDIA's H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 1980 MHz max SM clock, 989 TFLOP/s dense BF16."""
+    hbm_sheet = (3350.0, "H100 SXM data sheet (3.35 TB/s), not measured")
+    tensor_sheet = (989.0, "H100 SXM data sheet (989 TFLOP/s dense BF16), not measured")
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
+    p = {}
     if os.path.exists(path):
         with open(path) as fh:
             p = json.load(fh)
-        return (float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)", float(p.get("sm_max_mhz", 1965.0)),
-                float(p.get("bf16_tflops", 1590.0)))
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)", 1965.0, 1590.0
+    hbm = (float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)") if "hbm_gbs" in p else hbm_sheet
+    tensor = ((float(p["bf16_tflops"]), "measured (MEASURED_PEAKS.json bf16_tflops)") if "bf16_tflops" in p
+              else tensor_sheet)
+    return hbm[0], hbm[1], float(p.get("sm_max_mhz", 1980.0)), tensor[0], tensor[1]
 
 
 class ClockSampler:
@@ -264,6 +277,9 @@ def run_reference(args):
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
+    if args.dump_outputs:
+        print("bench.py: --dump-outputs is ignored with --impl reference (it times the reference's CPU algorithm on "
+              "a sample of the clouds, not the native path)", file=sys.stderr)
     import torch
     run = oracle_layer(len(os.sched_getaffinity(0)))
     clouds = 4
@@ -359,11 +375,24 @@ def sparse_aggregate_block(dev, steps=10):
            "ms": ms, "edges_per_s": E / (ms * 1e-3), "steps": steps,
            "roofline": {"bound": "hbm", "achieved": gather_bytes / (ms * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
                         "frac": gather_bytes / (ms * 1e-3) / 1e9 / peak, "bytes_per_launch": gather_bytes,
-                        "model": "gather model: 4C+4 B/edge + (8C+4) B/node (SURVEY.md 8d); ncu dram bytes of the same "
-                                 "launch: profiles/r02_aggregate_products_ncu.json"}}
+                        "model": "gather model: 4C+4 B/edge + (8C+4) B/node (SURVEY.md 8d)"}}
     del x, out, flush, csr
     torch.cuda.empty_cache()
     return res
+
+
+def dump_output(directory, y, rank, world):
+    """One GPU: the whole output as DIR/y.npy.  N GPUs: every rank writes its shard as DIR/y_rank<r>.npy, as a fixed
+    sample (every s-th element of the flattened shard) where the shards together would exceed 64 MB."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    y = y.float()
+    if world == 1:
+        np.save(os.path.join(directory, "y.npy"), y.cpu().numpy())
+        return
+    cap = (64 << 20) // 4 // world
+    stride = -(-y.numel() // cap)
+    np.save(os.path.join(directory, "y_rank%d.npy" % rank), (y if stride == 1 else y.reshape(-1)[::stride]).cpu().numpy())
 
 
 def _claim_stdout():
@@ -419,12 +448,16 @@ def run_native(args):
             # host-side launch work: without the head start the first-launch latency after the synchronize is 5-15 %
             # of a 20-step region; the `sustained` block below is the same loop over ~2 s without any of this)
             torch.cuda._sleep(4_000_000)
+            y_last = None
             beg.record()
             for i in range(args.steps):
-                mod(xs[i % N_ROTATE])
+                y_last = mod(xs[i % N_ROTATE])
             end.record()
             barrier()
         ms = beg.elapsed_time(end)
+        if args.dump_outputs and y_last is not None:
+            dump_output(args.dump_outputs, y_last, rank, world)
+        del y_last
         knn_ms, knn_n = _native.kernel_timing_read("knn")
         _native.kernel_timing(False)
 
@@ -513,16 +546,12 @@ def run_native(args):
             dist.destroy_process_group()
         return
 
-    peak, peak_src, sm_max, tensor_peak = peaks()
+    peak, peak_src, sm_max, tensor_peak, tensor_src = peaks()
     kernel_ms = knn_ms / max(knn_n, 1)
     hbm_achieved = EDGES_PER_STEP * ALGO_BYTES_PER_EDGE / (kernel_ms * 1e-3) / 1e9
     tensor_flop = 2.0 * B * N * N * (3 * C + 16)     # 3 split products hi*hi, hi*mid, mid*hi over C channels + one K=16 block folding -|x_j|^2/2
     achieved = tensor_flop / (kernel_ms * 1e-3) / 1e12
     traffic = None
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tpath):
-        with open(tpath) as fh:
-            traffic = json.load(fh).get("knn_tc4_kernel")
     clk = clocks.summary()
     out = {
         "metric": "edges/sec EdgeConv fwd (B=16,N=4096,k=20,C=64)",
@@ -531,7 +560,7 @@ def run_native(args):
         "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "f32", "data": "synthetic",
         "config": {"workload": WORKLOAD, "edges_per_step_per_gpu": EDGES_PER_STEP, "parallelism": "batch-sharded x%d" % world,
-                   "l2": "inputs rotate over %d distinct 16.8 MB batches (134 MB > 126 MB L2)" % N_ROTATE,
+                   "l2": "inputs rotate over %d distinct 16.8 MB batches (134 MB > 50 MB L2)" % N_ROTATE,
                    "queue": "the K timed steps are enqueued behind a ~2 ms spin kernel (device-side throughput; CUDA events "
                             "bracket exactly the K steps)",
                    "host_binding": numa},
@@ -540,19 +569,18 @@ def run_native(args):
                 "ms_per_step": ms_e2e / args.steps},
         "gpu_launches": 4 * args.steps,   # pack weights, fused prologue + node GEMM, tensor-core selection + consumer, exact completion
         "clocks": clk,
-        # What binds the dominant kernel: the tcgen05 pre-filter and the CUDA-core top-k bookkeeping that drains its
-        # accumulators (tensor pipe + ALU issue).  `frac` is against the measured bf16 tensor peak; the HBM fraction
-        # the metric asks for is kept as a secondary block - the kernel is nowhere near HBM bound.
+        # What binds the dominant kernel: the wgmma pre-filter and the CUDA-core top-k bookkeeping that drains its
+        # accumulators (tensor pipe + ALU issue).  `frac` is against the bf16 tensor peak; the HBM fraction the
+        # metric asks for is kept as a secondary block - the kernel is nowhere near HBM bound.
         "roofline": {"bound": "tensor", "co_bound": "alu (top-k filter / list maintenance next to the tensor pipe)",
-                     "kernel": "knn_tc4_kernel<28> (four query tiles per CTA: producer warps (TMA ring + tcgen05 "
-                               "bf16 (hi,mid) pre-filter) + 16 filter warps with sorting-network list merges, set "
-                               "membership by interval arithmetic with exact fp32 chains in the ambiguous band, "
-                               "certificate, fused EdgeConv gather/max)",
+                     "kernel": "knn_tc4_kernel<28> (two query tiles per CTA: a TMA producer warp + two filter "
+                               "warpgroups, each running its wgmma bf16 (hi,mid) pre-filter and sorting-network list "
+                               "merges, set membership by interval arithmetic with exact fp32 chains in the ambiguous "
+                               "band, certificate, fused EdgeConv gather/max)",
                      "achieved": achieved, "peak": tensor_peak, "unit": "TFLOP/s", "frac": achieved / tensor_peak,
                      "flop_per_launch": tensor_flop, "traffic": traffic,
-                     "traffic_source": "profiles/traffic.json (ncu --set full dram__bytes_read.sum + dram__bytes_write.sum of "
-                                       "one launch; not re-measured in this run)",
-                     "peak_source": "measured (MEASURED_PEAKS.json bf16_tflops, burst)", "kernel_ms": kernel_ms,
+                     "traffic_source": "not measured",
+                     "peak_source": tensor_src, "kernel_ms": kernel_ms,
                      "kernel_share_of_step": kernel_ms / (ms / args.steps),
                      "hbm": {"achieved": hbm_achieved, "peak": peak, "unit": "GB/s", "frac": hbm_achieved / peak,
                              "peak_source": peak_src,

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Model-level timing of BASELINE configs 2 and 3 on one B200 (secondary; bench.py is the
-driver's contract): the reference's model assembly restated on top of the drop-in classes.
+"""Model-level timing of BASELINE configs 2 and 3 on one H100 (secondary; bench.py is the
+headline benchmark): the reference's model assembly restated on top of the drop-in classes.
 
   c2  ResGCN-28 (examples/sem_seg_dense/architecture.py:7-56): DenseDilatedKnnGraph + head
       GraphConv2d + 27 ResDynBlock2d (dilation 1..27) + fusion / prediction BasicConvs,

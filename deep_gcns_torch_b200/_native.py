@@ -1,4 +1,4 @@
-"""ctypes binding of the C ABI in include/dgcn.h (libdgcn.so, sm_100a kernels).
+"""ctypes binding of the C ABI in include/dgcn.h (libdgcn.so, sm_90a kernels).
 
 PyTorch is only the carrier here: it owns device memory (inputs, outputs and the
 scratch workspace handed to the library) and the stream the kernels are put on.
@@ -127,6 +127,10 @@ def _declare(lib):
     lib.dgcn_debug_kernel_timing_read.restype = ctypes.c_int
     lib.dgcn_debug_kernel_timing_read.argtypes = [ctypes.c_char_p, ctypes.POINTER(ctypes.c_double),
                                                   ctypes.POINTER(c_i64)]
+    lib.dgcn_debug_tc_certification.restype = ctypes.c_int
+    lib.dgcn_debug_tc_certification.argtypes = [c_i32]
+    lib.dgcn_debug_tc_certification_read.restype = ctypes.c_int
+    lib.dgcn_debug_tc_certification_read.argtypes = [ctypes.POINTER(c_i64), ctypes.POINTER(c_i64)]
     lib.dgcn_gather_rows.restype = ctypes.c_int
     lib.dgcn_gather_rows.argtypes = [vp, c_i64, vp, c_i64, vp, vp]
 
@@ -162,7 +166,7 @@ def _ptr(t):
 def _require_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:
-            raise RuntimeError("deep_gcns_torch_b200 runs on CUDA tensors only (sm_100a kernels, no CPU fallback); "
+            raise RuntimeError("deep_gcns_torch_b200 runs on CUDA tensors only (sm_90a kernels, no CPU fallback); "
                                "got a tensor on %s" % t.device)
 
 
@@ -496,7 +500,7 @@ def linear_residual_supported(K, M):
 
 
 def linear_residual(a, weight, bias=None, res=None, out=None):
-    """dgcn_linear_residual: out (N, M) = a @ weight^T (+ bias) (+ res) on the tcgen05 tensor cores."""
+    """dgcn_linear_residual: out (N, M) = a @ weight^T (+ bias) (+ res) on the tensor cores (wgmma)."""
     _require_cuda(a, weight, bias, res, out)
     a, weight, bias, res = _f32(a), _f32(weight), _f32(bias), _f32(res)
     N, K = a.shape
@@ -542,10 +546,24 @@ def kernel_timing_read(tag):
     return ms.value, n.value
 
 
+def tc_certification(enable):
+    """Count the queries the tensor-core pre-filter leaves uncertified (dgcn_debug_tc_certification; synchronises
+    after every selection while enabled)."""
+    return lib().dgcn_debug_tc_certification(int(bool(enable)))
+
+
+def tc_certification_read():
+    """(uncertified queries, queries) since the last read."""
+    failed, total = c_i64(0), c_i64(0)
+    _check(lib().dgcn_debug_tc_certification_read(ctypes.byref(failed), ctypes.byref(total)),
+           "dgcn_debug_tc_certification_read")
+    return failed.value, total.value
+
+
 def set_knn_path(path):
     """A/B switch for tests and measurements: 'ffma' makes the calls of THIS thread pass
     DGCN_KNN_EXACT_FP32 (fp32 FMA selection kernels only); 'tc1' passes DGCN_KNN_TC_TILE_PER_CTA (tensor-core
-    pre-filter, always the one-tile-per-CTA kernel); 'tc' / 'auto' = the default routing (tcgen05 pre-filter +
-    exact re-rank where the shape allows, four query tiles per CTA where that kernel applies).  The library
+    pre-filter, always the one-tile-per-CTA kernel); 'tc' / 'auto' = the default routing (tensor-core pre-filter +
+    exact re-rank where the shape allows, several query tiles per CTA where that kernel applies).  The library
     holds no state."""
     _knn_flags.value = {"ffma": KNN_EXACT_FP32, "tc1": KNN_TC_TILE_PER_CTA, "tc": 0, "auto": 0}[path]

@@ -1,7 +1,6 @@
-"""In-tree build of the sm_100a kernels into deep_gcns_torch_b200/lib/libdgcn.so.
+"""In-tree build of the sm_90a kernels into deep_gcns_torch_b200/lib/libdgcn.so.
 
-nvcc cross-compiles without a GPU; the .so is git-ignored but travels to the GPU
-box with the repo snapshot.  `python -m deep_gcns_torch_b200.build` rebuilds.
+nvcc cross-compiles without a GPU; the .so is a build product (git-ignored).  `python -m deep_gcns_torch_b200.build` rebuilds.
 """
 import hashlib
 import os
@@ -13,8 +12,8 @@ CSRC = os.path.join(PKG, "csrc")
 LIBDIR = os.path.join(PKG, "lib")
 LIB = os.path.join(LIBDIR, "libdgcn.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
-         "-Xcompiler", "-fPIC"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
 
 
 def sources():
@@ -50,7 +49,7 @@ def build(force=False, verbose=False):
             print(out)
         if p.returncode != 0:
             raise RuntimeError("nvcc failed: %s\n%s" % (" ".join(cmd), out))
-    cmd = [NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [NVCC, "-shared", "-o", LIB] + objs + ARCH
     subprocess.run(cmd, check=True)
     for o in objs:
         os.remove(o)

@@ -1,4 +1,4 @@
-// Shared device helpers for the dgcn kernels (sm_100a).
+// Shared device helpers for the dgcn kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -45,6 +45,15 @@ void set_last_cuda_error(cudaError_t e, const char* file, int line);
       if (slot__) smem_set__[dev__].store(want__, std::memory_order_relaxed);                        \
     }                                                                                                \
   } while (0)
+
+// SM count and L2 size of the current device (write-once per-device cache of what the driver reports; 132 SMs and
+// 50 MB, an H100 SXM, if the query fails).  Grid and slab sizes derive from them.
+int device_sm_count();
+size_t device_l2_bytes();
+
+// Certification counters of the tensor-core kNN pre-filter (see dgcn_debug_tc_certification).
+bool debug_certification_on();
+void debug_certification_add(int64_t uncertified, int64_t queries);
 
 // Optional event bracket around a path's dominant kernel (see dgcn_debug_kernel_timing).
 struct KernelTimer {

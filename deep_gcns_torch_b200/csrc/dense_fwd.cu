@@ -20,16 +20,18 @@ __global__ void to_node_major_kernel(const float* __restrict__ x, int64_t sb, in
                                      float* __restrict__ xt);
 
 // ---- launch helpers for the selection kernels -------------------------------------
+// Clouds per slab of distance rows: two slabs are in flight (rows of slab s+1 under the select of slab s), so each
+// gets half of the L2 (at least one cloud).
 static size_t knn_slab_clouds(int64_t B, int64_t N) {
   const int64_t ldd = (N + 3) / 4 * 4;
   const int64_t per_cloud = N * ldd * 4;
-  int64_t nb = (96ll << 20) / (per_cloud > 0 ? per_cloud : 1);
+  int64_t nb = static_cast<int64_t>(device_l2_bytes() / 2) / (per_cloud > 0 ? per_cloud : 1);
   if (nb < 1) nb = 1;
   if (nb > B) nb = B;
   return static_cast<size_t>(nb);
 }
 
-constexpr int TC_FALLBACK_GRID = 148;  // CTAs of the exact completion kernel (one uncertified query at a time each)
+constexpr int TC_FALLBACK_GRID = 132;  // CTAs of the exact completion kernel (one uncertified query at a time each; H100 SXM SMs)
 
 static bool tc_shape_ok(int64_t C, int64_t N, int64_t K) {
   return K <= TC_K_MAX && C <= TC_MAX_C && N >= TILE && (N % TILE) == 0;
@@ -98,7 +100,7 @@ static EncodeTiledFn tensor_map_encoder() {
 }
 // bf16 matrix (rows, cols) row-major -> tensor map with boxes of 64 columns (128 bytes) x box_rows rows, SWIZZLE_128B:
 // a box lands in shared memory as box_rows x 128 B rows with the 16-byte chunks XOR-swizzled by (row & 7), which is
-// the canonical MN-major UMMA layout of one 64-wide MN block.
+// the canonical MN-major wgmma layout of one 64-wide MN block.
 static int make_plane_map(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int box_rows) {
   EncodeTiledFn enc = tensor_map_encoder();
   if (!enc) return DGCN_ERR_UNSUPPORTED;
@@ -167,7 +169,7 @@ static int launch_knn_tc(KnnArgs& a, Workspace& ws, cudaStream_t stream, const f
     t.work_bytes = static_cast<int>(tc_work_bytes(kp, a.k, t.wide != 0, nch));
     const size_t smem = static_cast<size_t>(t.work_bytes) + sizeof(TcTail) + 1024;
     const bool packed = N <= 4096;
-    // four query tiles per CTA, warp specialised (knn_tc4.cuh), where its smaller work area and fixed consumer fit
+    // T4_GROUPS query tiles per CTA, warp specialised (knn_tc4.cuh), where its smaller work area and fixed consumer fit
     const bool train = a.epi.mode == EPI_EDGE && a.epi.norm == DGCN_NORM_BATCH_TRAIN;
     const bool quad = !a.tc_tile_per_cta && packed && t.wide && !train && t.xt32 && (C & 7) == 0 && knn_tc4_list_ok(kp, a.k);
     int rc;
@@ -185,6 +187,12 @@ static int launch_knn_tc(KnnArgs& a, Workspace& ws, cudaStream_t stream, const f
     float* extra = a.epi.partial ? a.epi.partial + n_cta * 2 * a.epi.c_out : nullptr;
     knn_exact_rows_kernel<<<TC_FALLBACK_GRID, 256, 0, stream>>>(a, t.fail_count, t.fail_list, extra);
     DGCN_LAUNCH_CHECK();
+    if (debug_certification_on()) {
+      int failed = 0;
+      DGCN_CUDA_TRY(cudaMemcpyAsync(&failed, t.fail_count, sizeof(int), cudaMemcpyDeviceToHost, stream));
+      DGCN_CUDA_TRY(cudaStreamSynchronize(stream));
+      debug_certification_add(failed, static_cast<int64_t>(B) * N);
+    }
   }
   if (n_partial) *n_partial = n_cta + TC_FALLBACK_GRID;
   return DGCN_OK;
@@ -213,7 +221,7 @@ int launch_knn(KnnArgs& a, Workspace& ws, cudaStream_t stream, int64_t* n_partia
   if (knn_takes_tc(a))
     return launch_knn_tc(a, ws, stream, a.epi.mode == EPI_MR ? a.epi.xt : nullptr, n_partial, pqf);
   if (pqf) return DGCN_ERR_BAD_ARG;   // (internal misuse) nobody would produce PQ
-  const bool rows_on_tc = K > 32 && K <= LARGE_K_MAX && dist_rows_tc_ok(a);   // large-K: distance rows on tcgen05
+  const bool rows_on_tc = K > 32 && K <= LARGE_K_MAX && dist_rows_tc_ok(a);   // large-K: distance rows on the tensor cores
   __nv_bfloat16* planes3 = nullptr;
   if (rows_on_tc) {
     planes3 = ws.take<__nv_bfloat16>(dist_rows_tc_plane_elems(B, a.C, N));
@@ -319,7 +327,8 @@ int launch_knn(KnnArgs& a, Workspace& ws, cudaStream_t stream, int64_t* n_partia
       select_rows_fast_kernel<<<static_cast<unsigned>(ceil_div(rows, warps_f)), warps_f * 32, smem_f, st>>>(
           a, b0, nb, drows_s, ldd, cap, sample_rank, warps_f, rowlist_s, rowlist_s + 64);
       DGCN_LAUNCH_CHECK();
-      select_rows_kernel<<<296, warps * 32, smem, st>>>(a, b0, nb, drows_s, ldd, KP, ldd, warps, rowlist_s + 64, rowlist_s);
+      select_rows_kernel<<<2 * device_sm_count(), warps * 32, smem, st>>>(a, b0, nb, drows_s, ldd, KP, ldd, warps, rowlist_s + 64,
+                                                                      rowlist_s);   // grid-stride over the handed-over rows
       DGCN_LAUNCH_CHECK();
     } else {
       select_rows_kernel<<<static_cast<unsigned>(ceil_div(rows, warps)), warps * 32, smem, st>>>(

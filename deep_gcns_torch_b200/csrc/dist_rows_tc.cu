@@ -1,13 +1,12 @@
-// Distance rows of the large-K slab path on the tcgen05 tensor cores.
+// Distance rows of the large-K slab path on the Hopper tensor cores (wgmma).
 //
 //   D[i][j] = (|x_i|^2 + (-2 x_i.x_j)) + |x_j|^2        gcn_lib/dense/torch_edge.py:32-42 (pairwise_distance)
 //
 // for all pairs of one cloud, written as fp32 rows of the L2-sized slab that select_rows_fast_kernel consumes
-// (K = k * dilation > 48: the 25 dilated layers of ResGCN-28).  The fp32 tile engine (dist_rows_kernel) spends
-// 56 us per 4096-point cloud on the N^2 C contraction at 77 % issue utilisation; here the contraction runs as a
-// THREE-plane bf16 split x = hi + mid + lo (24 bits: the split is exact) with the six products
+// (K = k * dilation > 48: the 25 dilated layers of ResGCN-28).  The contraction runs as a THREE-plane bf16 split
+// x = hi + mid + lo (24 bits: the split is exact) with the six products
 //   hi*hi, hi*mid, mid*hi, mid*mid, hi*lo, lo*hi
-// accumulated in fp32 in TMEM.  Dropped terms (mid*lo, lo*mid, lo*lo) are <= 2^-23 |x_i||x_j|; what remains is the
+// accumulated in fp32.  Dropped terms (mid*lo, lo*mid, lo*lo) are <= 2^-23 |x_i||x_j|; what remains is the
 // fp32 accumulation of exact bf16 products - an fp32-grade value of the same formula, closer to the fp64 distance
 // than a 64-step fp32 FMA chain, NOT bit-identical to it.  The ranking contract of the slab path is the oracle's:
 // equal to the reference on tie-free inputs, mismatches only between candidates whose fp64 distances differ by
@@ -15,17 +14,18 @@
 // call flag DGCN_KNN_EXACT_FP32 keeps the fp32 FMA rows.
 //
 // One CTA per (128 queries, chunk of candidate tiles) of a cloud - the candidate range is split so that one cloud
-// fills the 148 SMs -, 288 threads: warps 0-7 = epilogue (thread = TMEM lane = query row; two warps per lane quarter
-// take alternate 32-column blocks), warp 8 =
-// producer (one elected thread: TMA + MMA issue).  Query planes resident (3 x 16 KB), candidate tiles of 128 points
-// through a 2-stage ring (2 x 48 KB) by TMA (SWIZZLE_128B boxes = canonical MN-major UMMA layout, like knn_tc),
-// two 128-column TMEM accumulators: MMA(t+1) runs under the epilogue of tile t.  Epilogue: tcgen05.ld 32 columns,
-// transpose through a padded shared-memory stage, row-contiguous 128-byte stores of (sq_i + (-2 acc)) + sq_j.
+// fills the SMs -, 288 threads: warpgroups 0-1 = query rows 0..63 / 64..127 (wgmma m64n64k16 into registers,
+// epilogue straight from the accumulator fragments), warp 8 = producer (one elected thread: TMA).  Query planes
+// resident (3 x 16 KB), candidate tiles of 128 points through a 2-stage ring (2 x 48 KB) by TMA (SWIZZLE_128B boxes =
+// canonical MN-major wgmma layout, like knn_tc): the TMA of tile t+2 runs under the wgmma and epilogue of tile t+1.
+// Epilogue: each quad of lanes stores 8 consecutive floats (one 32-byte sector) of a row of
+// (sq_i + (-2 acc)) + sq_j.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
 #define DGCN_TEMPLATES_ONLY      // device helpers of knn_tc.cuh only: its kernels live in dense_fwd.cu
 #include "knn_tc.cuh"
+#include "wgmma.cuh"
 
 namespace dgcn {
 
@@ -65,9 +65,7 @@ struct DrArgs {
 struct DrBars {
   uint64_t q_full;            // query planes landed
   uint64_t tma_full[2];       // candidate stage s landed
-  uint64_t mma_done[2];       // MMAs into accumulator a completed (its stage is free, the accumulator readable)
-  uint64_t acc_free[2];       // the 256 epilogue threads have drained accumulator a
-  uint32_t tmem_base;
+  uint64_t stage_free[2];     // the 256 consumer threads have finished their wgmma on stage s
 };
 
 __global__ void __launch_bounds__(288, 1) dist_rows_tc_kernel(const __grid_constant__ DrArgs g) {
@@ -75,10 +73,9 @@ __global__ void __launch_bounds__(288, 1) dist_rows_tc_kernel(const __grid_const
   unsigned char* base = dr_smem + ((1024u - (smem_u32(dr_smem) & 1023u)) & 1023u);
   unsigned char* qs = base;                                        // [3 planes][2 MN][Cpad rows][128 B]
   unsigned char* cs = qs + DR_PLANES * DR_PLANE_BYTES;             // 2 stages of the same
-  float* stage = reinterpret_cast<float*>(cs + 2 * DR_PLANES * DR_PLANE_BYTES);     // [8 warps][32][33]
-  float* sqq_s = stage + 8 * 32 * 33;                                               // [128] |x_i|^2 of the queries
+  float* sqq_s = reinterpret_cast<float*>(cs + 2 * DR_PLANES * DR_PLANE_BYTES);   // [128] |x_i|^2 of the queries
   DrBars& bar = *reinterpret_cast<DrBars*>(sqq_s + TILE);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5;
   const int N = g.N, Cpad = g.Cpad;
   const int bl = blockIdx.z, b = g.b0 + bl, q0 = blockIdx.x * TILE;
   const int ntiles = (N / TILE) / static_cast<int>(gridDim.y);          // candidate tiles of this CTA
@@ -89,21 +86,16 @@ __global__ void __launch_bounds__(288, 1) dist_rows_tc_kernel(const __grid_const
     mbar_init(&bar.q_full, 1);
     for (int i = 0; i < 2; ++i) {
       mbar_init(&bar.tma_full[i], 1);
-      mbar_init(&bar.mma_done[i], 1);
-      mbar_init(&bar.acc_free[i], 256);
+      mbar_init(&bar.stage_free[i], 256);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (tid < TILE) sqq_s[tid] = __ldg(g.sq + static_cast<int64_t>(b) * N + q0 + tid);
-  if (warp == 0) tmem_alloc(&bar.tmem_base, 256);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = bar.tmem_base;
 
   if (warp == 8) {
-    if (lane == 0) {
-      // ===================== producer: TMA + MMA issue =======================================================
+    if ((tid & 31) == 0) {
+      // ===================== producer: TMA =====================================================================
       auto tma_tile = [&](unsigned char* dst, int p0, uint64_t* mb) {
         mbar_expect_tx(mb, static_cast<uint32_t>(DR_PLANES * plane_bytes));
         for (int pl = 0; pl < DR_PLANES; ++pl)
@@ -114,64 +106,55 @@ __global__ void __launch_bounds__(288, 1) dist_rows_tc_kernel(const __grid_const
       tma_tile(qs, q0, &bar.q_full);
       tma_tile(cs, tile0 * TILE, &bar.tma_full[0]);
       if (ntiles > 1) tma_tile(cs + DR_PLANES * plane_bytes, (tile0 + 1) * TILE, &bar.tma_full[1]);
-      mbar_wait(&bar.q_full, 0u);
-      const int pa[6] = {0, 0, 1, 1, 0, 2};   // hi*hi, hi*mid, mid*hi, mid*mid, hi*lo, lo*hi
-      const int pb[6] = {0, 1, 0, 1, 2, 0};
-      for (int t = 0; t < ntiles; ++t) {
+      // the stage of tile t is free once both warpgroups' wgmma on it have completed: refill it with tile t + 2
+      for (int t = 0; t + 2 < ntiles; ++t) {
         const int s = t & 1;
-        mbar_wait(&bar.tma_full[s], static_cast<uint32_t>((t >> 1) & 1));
-        if (t >= 2) mbar_wait(&bar.acc_free[s], static_cast<uint32_t>(((t - 2) >> 1) & 1));
-        tc_fence_after();
-        const uint32_t abase = smem_u32(qs), bbase = smem_u32(cs + s * DR_PLANES * plane_bytes);
-        const uint32_t d = tmem + static_cast<uint32_t>(s * TILE);
-        uint32_t accum = 0;
-        for (int kk = 0; kk < Cpad / 16; ++kk) {
-#pragma unroll
-          for (int term = 0; term < 6; ++term) {
-            umma_bf16(d, umma_desc_mn_sw128(abase + pa[term] * plane_bytes + kk * 2048, Cpad * 128, 1024),
-                      umma_desc_mn_sw128(bbase + pb[term] * plane_bytes + kk * 2048, Cpad * 128, 1024),
-                      kIdescBf16MnMn128x128, accum);
-            accum = 1;
-          }
-        }
-        umma_commit(&bar.mma_done[s]);
-        // the stage of tile t is free once its MMAs have completed: refill it with tile t + 2
-        if (t + 2 < ntiles) {
-          mbar_wait(&bar.mma_done[s], static_cast<uint32_t>((t >> 1) & 1));
-          tma_tile(cs + s * DR_PLANES * plane_bytes, (tile0 + t + 2) * TILE, &bar.tma_full[s]);
-        }
+        mbar_wait(&bar.stage_free[s], static_cast<uint32_t>((t >> 1) & 1));
+        tma_tile(cs + s * DR_PLANES * plane_bytes, (tile0 + t + 2) * TILE, &bar.tma_full[s]);
       }
     }
   } else {
-    // ===================== epilogue: D = (sq_i + (-2 acc)) + sq_j, row-contiguous stores ==========================
-    float* st = stage + warp * 32 * 33;
-    const int quarter = warp & 3, half = warp >> 2;
+    // ===================== warpgroup wg: query rows 64 wg .. 64 wg + 63 =========================================
+    const int wg = warp >> 2;
+    const int pa[6] = {0, 0, 1, 1, 0, 2};   // hi*hi, hi*mid, mid*hi, mid*mid, hi*lo, lo*hi
+    const int pb[6] = {0, 1, 0, 1, 2, 0};
     const float* sqb = g.sq + static_cast<int64_t>(b) * N;
-    float* rows = g.drows + (static_cast<int64_t>(bl) * N + q0 + quarter * 32) * g.ldd;
+    float* rows = g.drows + (static_cast<int64_t>(bl) * N + q0 + wg * 64) * g.ldd;
+    const uint32_t abase = smem_u32(qs) + wg * (Cpad * 128);
+    mbar_wait(&bar.q_full, 0u);
     for (int t = 0; t < ntiles; ++t) {
       const int s = t & 1;
-      mbar_wait(&bar.mma_done[s], static_cast<uint32_t>((t >> 1) & 1));
-      tc_fence_after();
-      for (int cb = half * 32; cb < TILE; cb += 64) {
-        float v[32];
-        __syncwarp();
-        tmem_ld32(tmem + static_cast<uint32_t>(s * TILE + cb) + (static_cast<uint32_t>(quarter * 32) << 16), v);
+      mbar_wait(&bar.tma_full[s], static_cast<uint32_t>((t >> 1) & 1));
+      const uint32_t bbase = smem_u32(cs + s * DR_PLANES * plane_bytes);
+      float d0[32], d1[32];                 // candidates 0..63 / 64..127 of the tile
+      wg_fence();
+      for (int kk = 0; kk < Cpad / 16; ++kk) {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) st[lane * 33 + j] = v[j];
-        __syncwarp();
-        const int col = (tile0 + t) * TILE + cb + lane;
-        const float sqj = __ldg(sqb + col);
-#pragma unroll
-        for (int rr = 0; rr < 32; ++rr)
-          rows[static_cast<int64_t>(rr) * g.ldd + col] = (sqq_s[quarter * 32 + rr] + (-2.0f * st[rr * 33 + lane])) + sqj;
+        for (int term = 0; term < 6; ++term) {
+          const uint32_t acc = (kk | term) != 0 ? 1u : 0u;
+          const uint64_t da = wg_desc_sw128(abase + pa[term] * plane_bytes + kk * 2048, Cpad * 128, 1024);
+          const uint32_t bo = bbase + pb[term] * plane_bytes + kk * 2048;
+          wgmma_m64n64<1, 1>(d0, da, wg_desc_sw128(bo, Cpad * 128, 1024), acc);
+          wgmma_m64n64<1, 1>(d1, da, wg_desc_sw128(bo + Cpad * 128, Cpad * 128, 1024), acc);
+        }
       }
-      tc_fence_before();
-      mbar_arrive(&bar.acc_free[s]);
+      wg_commit();
+      wg_wait_all();
+      mbar_arrive(&bar.stage_free[s]);
+      const int col0 = (tile0 + t) * TILE;
+#pragma unroll
+      for (int i = 0; i < 32; i += 2) {
+        const int rr = wg_frag_row(i), c = col0 + wg_frag_col(i);
+        const float sqi = sqq_s[wg * 64 + rr];
+        const float2 sj0 = __ldg(reinterpret_cast<const float2*>(sqb + c));
+        const float2 sj1 = __ldg(reinterpret_cast<const float2*>(sqb + c + 64));
+        float* row = rows + static_cast<int64_t>(rr) * g.ldd;
+        *reinterpret_cast<float2*>(row + c) = make_float2((sqi + (-2.0f * d0[i])) + sj0.x, (sqi + (-2.0f * d0[i + 1])) + sj0.y);
+        *reinterpret_cast<float2*>(row + c + 64) =
+            make_float2((sqi + (-2.0f * d1[i])) + sj1.x, (sqi + (-2.0f * d1[i + 1])) + sj1.y);
+      }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem, 256);
 }
 
 typedef CUresult (*DrEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -225,10 +208,10 @@ int dist_rows_tc_launch(const KnnArgs& a, const __nv_bfloat16* planes, int b0, i
       return DGCN_ERR_CUDA;
   }
   g.sq = a.sq; g.drows = drows; g.b0 = b0; g.N = a.N; g.Cpad = cpad; g.ldd = ldd;
-  const size_t smem = static_cast<size_t>(3) * DR_PLANES * DR_PLANE_BYTES + 8 * 32 * 33 * 4 + TILE * 4 + sizeof(DrBars) + 1024;
+  const size_t smem = static_cast<size_t>(3) * DR_PLANES * DR_PLANE_BYTES + TILE * 4 + sizeof(DrBars) + 1024;
   DGCN_ENSURE_SMEM((dist_rows_tc_kernel), smem);
-  // split the candidate tiles of a query tile over CTAs until one launch fills the SMs (one CTA per SM: 162 KB smem)
-  int dev = 0, sms = 148;
+  // split the candidate tiles of a query tile over CTAs until one launch fills the SMs (one CTA per SM: 146 KB smem)
+  int dev = 0, sms = 0;
   DGCN_CUDA_TRY(cudaGetDevice(&dev));
   DGCN_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int ntiles = a.N / TILE;

@@ -302,7 +302,7 @@ __device__ __forceinline__ void cta_epilogue_wide(const KnnArgs& a, int b, int q
                                                   const unsigned char* ok, int* sel, int sel_ld, float* red,
                                                   int cta, int tid) {
   // tid: index of the calling thread inside the NW-warp team that owns the 128 queries (threadIdx.x when the
-  // team is the CTA; the four-tile kernel passes the index inside the warpgroup).  TRAIN syncs the whole CTA.
+  // team is the CTA; the multi-tile kernel passes the index inside the warpgroup).  TRAIN syncs the whole CTA.
   const Epilogue& e = a.epi;
   const int lane = tid & 31, warp = tid >> 5;
   const int N = a.N, k = a.k;

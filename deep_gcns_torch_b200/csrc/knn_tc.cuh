@@ -1,26 +1,24 @@
-// Tensor-core (tcgen05 / TMEM) path of the dilated kNN selection for K <= 48, C <= 64,
-// N % 128 == 0:  the N x N x C contraction runs on the 5th-gen tensor cores as a CERTIFIED
-// PRE-FILTER, the ranking itself stays exact fp32 (DESIGN.md 6).
+// Tensor-core (wgmma) path of the dilated kNN selection for K <= 48, C <= 64, N % 128 == 0:  the N x N x C
+// contraction runs on the Hopper tensor cores as a CERTIFIED PRE-FILTER, the ranking itself stays exact fp32
+// (DESIGN.md 6).
 //
 //   tc_prologue(_pq)  one pass over x: x = hi + mid (two bf16 planes, channel-major like x, channels
 //                     zero-padded to a multiple of 16; the three products hi*hi, hi*mid, mid*hi
 //                     reproduce x_i.x_j to ~2^-16 relative), |x|^2, the operand block that folds
 //                     -|x_j|^2/2 into the product, the node-major fp32 copy, max |x|^2 (and the
 //                     EdgeConv node GEMM).
-//   knn_tc_kernel     one 128-thread CTA = 128 queries of a cloud, two CTAs per SM.  Query planes stay
+//   knn_tc_kernel     one 128-thread CTA (one warpgroup) = 128 queries of a cloud.  Query planes stay
 //                     resident in shared memory; candidate tiles of 128 points are brought in by TMA
 //                     (cp.async.bulk.tensor, 64-point x Cpad-channel boxes with SWIZZLE_128B = the
-//                     canonical MN-major UMMA layout: x is channel-major = MN-major, so no
-//                     transposition anywhere, and no thread spends instructions on the copy).  Thread 0
-//                     issues the TMA of tile t+1 as soon as the MMAs of tile t have released the stage
-//                     and, from a poll at the next 16-column boundary of its filter loop, the
-//                     tcgen05.mma chain (M=128, N=128, K=16) of tile t+1 into the other of two TMEM
-//                     accumulators - so load and MMA of the next tile run under the filter of the
-//                     current one.  All 128 threads - thread r owns TMEM lane r = query r - filter the
-//                     finished accumulator (tcgen05.ld of 16 columns in flight while the previous 16 are
-//                     tested) against the thread's private threshold; survivors go to a private candidate buffer
+//                     canonical MN-major wgmma layout: x is channel-major = MN-major, so no
+//                     transposition anywhere, and no thread spends instructions on the copy).  Per
+//                     64-candidate block the warpgroup runs two m64n64k16 wgmma chains (query rows 0..63 and
+//                     64..127) and puts the accumulators into a shared-memory stage, row = query; the TMA
+//                     of tile t+1 is started as soon as the last wgmma of tile t has completed and lands
+//                     under the filter.  Thread r = query r filters its row in 16-column chunks against the
+//                     thread's private threshold; survivors go to a private candidate buffer
 //                     and from there into the query's register-resident sorted list of the KP best
-//                     APPROXIMATE keys (no atomics, no CTA barriers in the filter).
+//                     APPROXIMATE keys (no atomics in the filter).
 //                     Afterwards each thread re-evaluates its KP candidates with the exact fp32
 //                     FMA chain (same values as knn_small_kernel), sorts them, and certifies:
 //                       exact_K-th + eps < approx_KP-th     (eps = bound on |approx - exact|)
@@ -32,6 +30,7 @@
 #include <cuda.h>          // CUtensorMap (type only: the encoder comes from cudaGetDriverEntryPoint)
 #include <cuda_bf16.h>
 #include "knn.cuh"
+#include "wgmma.cuh"
 
 namespace dgcn {
 
@@ -133,104 +132,6 @@ __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src)
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {   // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {         // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, bf16 x bf16 -> fp32, one thread issues for the CTA
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp gets lane (base+i)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// 32 lanes x 16 consecutive fp32 columns, NOT waited for: the registers are valid only after tmem_wait16 on them
-__device__ __forceinline__ void tmem_ld16_async(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-// tcgen05.wait::ld; the registers are in/out operands so that no use (or copy) of them is scheduled above the wait
-__device__ __forceinline__ void tmem_wait16(uint32_t (&r)[16]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                 "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-               :
-               : "memory");
-}
-
-// 32 lanes x 8 consecutive fp32 columns, NOT waited for (see tmem_ld16_async)
-__device__ __forceinline__ void tmem_ld8_async(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];\n"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_wait8(uint32_t (&r)[8]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7])
-               :
-               : "memory");
-}
-
-// Shared-memory matrix descriptor, MN-major operand, SWIZZLE_128B (cute::UMMA::SmemDescriptor):
-// [0,14) start>>4 | [16,30) leading-dim byte offset>>4 = stride between 128-byte MN blocks |
-// [32,46) stride byte offset>>4 = stride between groups of 8 K rows | [46,48) version=1 |
-// [61,64) layout = 2 (SWIZZLE_128B).
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr, uint32_t mn_block_stride,
-                                                       uint32_t k_group_stride) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);
-  d |= static_cast<uint64_t>((mn_block_stride >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>((k_group_stride >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-// Instruction descriptor (cute::UMMA::InstrDescriptor): c=F32 [4,6)=1, a=BF16 [7,10)=1,
-// b=BF16 [10,13)=1, a_major=MN bit15, b_major=MN bit16, N>>3 [17,23), M>>4 [24,29).
-constexpr uint32_t kIdescBf16MnMn128x128 =
-    (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((128u >> 3) << 17) | ((128u >> 4) << 24);
-
 // ---- operand split ----------------------------------------------------------------------------
 // planes (B, TC_PLANES, Cpad, N) bf16: x = hi + mid with |mid| <= 2^-8 |x| and |x - hi - mid| <= 2^-17 |x|;
 // channels >= C are zero.  Three bf16 products hi*hi, hi*mid, mid*hi reproduce x_i.x_j to
@@ -379,8 +280,7 @@ __global__ void __launch_bounds__(256, 4) tc_prologue_pq_kernel(const float* __r
   // 128-wide pass
   const int tx = tid & 15, ty = tid >> 4;
   for (int m0 = 0; m0 < M; m0 += 128) {
-    // two outputs per instruction (fma.rn.f32x2: each half is the IEEE fma of the scalar code, so the chain per
-    // output - c ascending from 0 - and its bits are those of node_pq_kernel); the kernel is issue bound, not FMA-pipe bound
+    // the chain per output - c ascending from 0 - and its bits are those of node_pq_kernel
     float2 acc[4][4];
 #pragma unroll
     for (int i = 0; i < 4; ++i)
@@ -396,7 +296,10 @@ __global__ void __launch_bounds__(256, 4) tc_prologue_pq_kernel(const float* __r
 #pragma unroll
       for (int i = 0; i < 4; ++i)
 #pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = __ffma2_rn(make_float2(av[i], av[i]), wv[j], acc[i][j]);
+        for (int j = 0; j < 4; ++j) {
+          acc[i][j].x = fmaf(av[i], wv[j].x, acc[i][j].x);
+          acc[i][j].y = fmaf(av[i], wv[j].y, acc[i][j].y);
+        }
     }
     const float4 b0 = __ldg(reinterpret_cast<const float4*>(g.bk + m0 + tx * 4));
     const float4 b1 = __ldg(reinterpret_cast<const float4*>(g.bk + m0 + 64 + tx * 4));
@@ -415,11 +318,11 @@ __global__ void __launch_bounds__(256, 4) tc_prologue_pq_kernel(const float* __r
 
 
 // ---- the tensor-core kernel ------------------------------------------------------------------------
-// 256-bit read-only global load (sm_100: LDG.E.256); p must be 32-byte aligned
-__device__ __forceinline__ void ldg256(const float* p, float (&w)[8]) {
-  asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=f"(w[0]), "=f"(w[1]), "=f"(w[2]), "=f"(w[3]), "=f"(w[4]), "=f"(w[5]), "=f"(w[6]), "=f"(w[7])
-               : "l"(p));
+// eight consecutive floats as two 128-bit read-only loads; p must be 16-byte aligned
+__device__ __forceinline__ void ldg_f8(const float* p, float (&w)[8]) {
+  const float4 u = __ldg(reinterpret_cast<const float4*>(p)), v = __ldg(reinterpret_cast<const float4*>(p) + 1);
+  w[0] = u.x; w[1] = u.y; w[2] = u.z; w[3] = u.w;
+  w[4] = v.x; w[5] = v.y; w[6] = v.z; w[7] = v.w;
 }
 
 struct TcArgs {
@@ -433,23 +336,22 @@ struct TcArgs {
   int Cpad;
   int wide;                      // consumer variant (cta_epilogue_wide)
   int work_bytes;                // size of the work area, see tc_work_bytes
-  int xt32;                      // xt is 32-byte aligned: 256-bit row loads in the exact re-rank
+  int xt32;                      // xt is 32-byte aligned: 8-float row loads in the exact re-rank
   int flush_early, flush_late;   // packed path: buffered candidates per lane that trigger a flush (tiles 0-1 / later)
   int* fail_count;               // device counter
   int* fail_list;                // (B*N) encoded b*N + q
 };
 
-constexpr int TC_THREADS = 128;                       // one warpgroup: thread r = TMEM lane r = query r
+constexpr int TC_THREADS = 128;                       // one warpgroup: thread r = query r
 constexpr int TC_FLUSH_AT = 1;                        // unpacked (8-byte entries): flush whenever a lane buffered anything
 constexpr int TC_BUF = 16;                            // 8-byte slots per thread, >= TC_FLUSH_AT - 1 + 16 (checked every 16 columns)
 constexpr int TC_FLUSH_EARLY = 16;                    // packed 4-byte entries: 32 slots; tight threshold while the
 constexpr int TC_FLUSH_LATE = 16;                     // list still moves a lot (first tiles), fuller batches afterwards
 constexpr int TC_STAGE_BYTES = TC_PLANES * 2 * TC_MAX_C * 128;   // 32 KB: planes x 2 MN blocks x 64 rows x 128 B
 constexpr int TC_XBLOCK_BYTES = 2 * 16 * 128;                    // 4 KB: one extra K=16 block, 2 MN blocks x 16 rows x 128 B
-constexpr int TC_ISSUE_CHUNK = 2;                                 // 32-column chunk of tile t before which the MMAs of tile t+1 are issued
+constexpr int TC_ACC_LD = 68;                                     // accumulator stage: 64 columns + 4 (conflict-free row reads)
 
-// Shared memory of one CTA (128 queries of one cloud).  Several CTAs share an SM so that the
-// latency-bound phases of one (exact re-rank, neighbour gather) overlap the streaming phase of another.
+// Shared memory of one CTA (128 queries of one cloud).
 //   work (1024-aligned, work_bytes): while streaming [query planes 32 KB | candidate stage 32 KB |
 //   query extra block 4 KB | candidate extra block 4 KB], all canonical MN-major SWIZZLE_128B:
 //   [plane][mn_block(2)][Cpad rows][128 B]; the extra K=16 blocks hold ones (query side, rows 0..2) and the
@@ -458,11 +360,9 @@ constexpr int TC_ISSUE_CHUNK = 2;                                 // 32-column c
 //   tail: the fixed-size part below.
 struct TcTail {
   uint64_t cbuf[TC_BUF * TC_THREADS];               // 16 KB private candidate buffers, slot-major
-  uint64_t mbar;                                    // MMA of a tile has completed (tcgen05.commit)
-  uint64_t mbar_drained;                            // all 128 threads have finished reading the accumulator the next MMA overwrites
+  float acc[TILE][TC_ACC_LD];                       // 34 KB: one 128-query x 64-candidate accumulator block, row = query
   uint64_t mbar_tma;                                // the next tile's operands have landed (TMA complete_tx)
   uint64_t mbar_q;                                  // query planes + tile 0 have landed
-  uint32_t tmem_base;
   unsigned char ok[TILE];
 };
 
@@ -506,14 +406,14 @@ __device__ __forceinline__ void reg_insert_packed(uint32_t (&k)[KP], uint32_t nk
 }
 
 template <int KP, bool PACKED>
-__global__ void __launch_bounds__(TC_THREADS, 2) knn_tc_kernel(const __grid_constant__ TcArgs t) {
+__global__ void __launch_bounds__(TC_THREADS, 1) knn_tc_kernel(const __grid_constant__ TcArgs t) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   // SWIZZLE_128B atoms must sit on 1024-byte boundaries of the shared address space
   unsigned char* work = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   TcTail& sm = *reinterpret_cast<TcTail*>(work + t.work_bytes);
   const KnnArgs& a = t.a;
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const int r = tid;                                    // query row = TMEM lane
+  const int tid = threadIdx.x;
+  const int r = tid;                                    // query row
   const int b = blockIdx.y, q0 = blockIdx.x * TILE;
   const int N = a.N, Cpad = t.Cpad;
   const int plane_bytes = 2 * Cpad * 128;
@@ -525,8 +425,6 @@ __global__ void __launch_bounds__(TC_THREADS, 2) knn_tc_kernel(const __grid_cons
     // the TMA descriptors live in kernel-parameter space: fetch them into the descriptor cache before the first load
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&t.tm_planes)) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&t.tm_sqp)) : "memory");
-    mbar_init(&sm.mbar, 1);
-    mbar_init(&sm.mbar_drained, TC_THREADS);
     mbar_init(&sm.mbar_tma, 1);
     mbar_init(&sm.mbar_q, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -540,7 +438,7 @@ __global__ void __launch_bounds__(TC_THREADS, 2) knn_tc_kernel(const __grid_cons
     reinterpret_cast<uint4*>(qx)[ch] = make_uint4(one2, one2, one2, one2);
     reinterpret_cast<uint4*>(sx)[ch] = make_uint4(0u, 0u, 0u, 0u);        // rows 8..15 stay zero, TMA refreshes rows 0..7
   }
-  fence_proxy_async();                                    // generic-proxy fills above -> visible to TMA / tcgen05.mma
+  fence_proxy_async();                                    // generic-proxy fills above -> visible to TMA / wgmma
   __syncthreads();                                        // barriers initialised, fills done
   // One elected thread moves operands.  A tile = 2 planes x 2 MN blocks (boxes of 64 points x Cpad channels) plus
   // the 2 x (64 points x 8 rows) boxes of the -|x_j|^2/2 block.
@@ -563,40 +461,34 @@ __global__ void __launch_bounds__(TC_THREADS, 2) knn_tc_kernel(const __grid_cons
     tma_planes(stage, 0, &sm.mbar_q);
     tma_sx(0, &sm.mbar_q);
   }
-  if (warp == 0) {
-    __syncwarp();
-    tmem_alloc(&sm.tmem_base, 256);     // two 128-column accumulators
-  }
-  const uint32_t lane_base = static_cast<uint32_t>(warp * 32) << 16;
-  // One thread issues the 3 x Cpad/16 + 1 MMAs of a candidate tile into accumulator `buf` and commits.
-  auto issue_tile = [&](uint32_t tmem_acc) {
-    tc_fence_after();
-    const uint32_t abase = smem_u32(qstage), bbase = smem_u32(stage);
+  // The warpgroup multiplies the 128 queries against one 64-candidate MN block of the staged tile: rows 0..63 and
+  // 64..127 as two m64n64 chains of 3 x Cpad/16 + 1 wgmma each, then the accumulators go to the shared stage where
+  // thread r reads row r.
+  const uint32_t abase = smem_u32(qstage), bbase = smem_u32(stage);
+  auto mma_block = [&](int cb, float (&d0)[32], float (&d1)[32]) {
     const int pa[3] = {0, 0, 1};   // hi*hi, hi*mid, mid*hi  (mid*mid <= 2^-16 |x_i||x_j| is inside eps)
     const int pb[3] = {0, 1, 0};
+    wg_fence();
     uint32_t acc = 0;
+#pragma unroll 1
     for (int kk = 0; kk < Cpad / 16; ++kk) {
 #pragma unroll
       for (int term = 0; term < 3; ++term) {
-        const uint64_t da = umma_desc_mn_sw128(abase + pa[term] * plane_bytes + kk * 2048, Cpad * 128, 1024);
-        const uint64_t db = umma_desc_mn_sw128(bbase + pb[term] * plane_bytes + kk * 2048, Cpad * 128, 1024);
-        umma_bf16(tmem_acc, da, db, kIdescBf16MnMn128x128, acc);
+        const uint32_t ao = abase + pa[term] * plane_bytes + kk * 2048;
+        const uint64_t db = wg_desc_sw128(bbase + pb[term] * plane_bytes + cb * (Cpad * 128) + kk * 2048, Cpad * 128, 1024);
+        wgmma_m64n64<1, 1>(d0, wg_desc_sw128(ao, Cpad * 128, 1024), db, acc);
+        wgmma_m64n64<1, 1>(d1, wg_desc_sw128(ao + Cpad * 128, Cpad * 128, 1024), db, acc);
         acc = 1;
       }
     }
     // + 1 x (-|x_j|^2/2): the accumulator becomes x_i.x_j - |x_j|^2/2 = -key/2
-    umma_bf16(tmem_acc, umma_desc_mn_sw128(smem_u32(qx), 2048, 1024), umma_desc_mn_sw128(smem_u32(sx), 2048, 1024),
-              kIdescBf16MnMn128x128, 1u);
-    umma_commit(&sm.mbar);
+    const uint64_t dsx = wg_desc_sw128(smem_u32(sx) + cb * 2048, 2048, 1024);
+    wgmma_m64n64<1, 1>(d0, wg_desc_sw128(smem_u32(qx), 2048, 1024), dsx, 1u);
+    wgmma_m64n64<1, 1>(d1, wg_desc_sw128(smem_u32(qx) + 2048, 2048, 1024), dsx, 1u);
+    wg_commit();
+    wg_wait_all();
   };
-  tc_fence_before();
-  __syncthreads();                                        // TMEM base address published
-  tc_fence_after();
-  const uint32_t tmem = sm.tmem_base;
-  if (tid == 0) {
-    mbar_wait(&sm.mbar_q, 0u);
-    issue_tile(tmem);
-  }
+  mbar_wait(&sm.mbar_q, 0u);
 
   const int qg = q0 + r;
   // the KP best approximate keys, ascending, in registers
@@ -667,40 +559,18 @@ __global__ void __launch_bounds__(TC_THREADS, 2) knn_tc_kernel(const __grid_cons
     thr_acc = -0.5f * tau_f;                        // the filter compares accumulators: key <= tau  <=>  acc >= -tau/2
   };
 
-  // Pipeline per tile t: wait MMA(t) -> everybody: "my reads of the other accumulator are done" (mbar_drained);
-  // thread 0: TMA of tile t+1 into the stage MMA(t) has just released -> filter accumulator t&1 in 16-column
-  // chunks (the tcgen05.ld of the next chunk in flight); at every chunk boundary thread 0 polls {TMA landed, all
-  // drained} and then issues MMA(t+1) into the other accumulator - nobody waits for it before the next tile.
+  // Per tile t and 64-candidate block cb: wgmma -> barrier (everybody has read the previous block out of the stage;
+  // after the last block, nobody reads the operand stage any more: thread 0 starts the TMA of tile t+1, which then
+  // lands under the filter) -> accumulators to the stage -> barrier -> thread r filters row r in 16-column chunks.
   for (int tile = 0; tile < ntiles; ++tile) {
-    const int par = tile & 1;
-    const bool more = tile + 1 < ntiles;
-    mbar_wait(&sm.mbar, static_cast<uint32_t>(par));
-    tc_fence_after();
-    bool to_issue = more && tid == 0;
-    if (more) {
-      tc_fence_before();                 // my tcgen05.ld of accumulator par^1 (tile-1) are complete and ordered
-      mbar_arrive(&sm.mbar_drained);
-      if (tid == 0) {
-        mbar_expect_tx(&sm.mbar_tma, tile_bytes);
-        tma_planes(stage, (tile + 1) * TILE, &sm.mbar_tma);
-        tma_sx((tile + 1) * TILE, &sm.mbar_tma);
-      }
-    }
-    // filter: thread = TMEM lane = query; the accumulator is -key/2 with key = |x_j|^2 - 2 x_i.x_j
+    if (tile > 0) mbar_wait(&sm.mbar_tma, static_cast<uint32_t>((tile - 1) & 1));
+    // filter: thread = query; the accumulator is -key/2 with key = |x_j|^2 - 2 x_i.x_j
     // (row-constant |x_i|^2 omitted): admit when acc >= -tau/2.  The query itself is an ordinary candidate here
     // even with exclude_self (it is dropped in the exact re-rank below; the list is 8 entries longer than K) -
     // a per-thread column patch would turn the chunk registers into an addressable local-memory array.
     const int j0 = tile * TILE;
-    const uint32_t tacc = tmem + static_cast<uint32_t>(par * TILE) + lane_base;
     const uint32_t flush_bytes = PACKED ? (tile < 2 ? t.flush_early : t.flush_late) * TC_THREADS * 4u
                                         : TC_FLUSH_AT * TC_THREADS * 8u;
-    auto poll_issue = [&]() {
-      if (to_issue && mbar_test(&sm.mbar_tma, static_cast<uint32_t>(par)) &&
-          mbar_test(&sm.mbar_drained, static_cast<uint32_t>(par))) {
-        issue_tile(tmem + static_cast<uint32_t>((par ^ 1) * TILE));
-        to_issue = false;
-      }
-    };
     // One 16-column chunk: test, buffer, flush when a lane's buffer runs full (checked once per chunk).  A macro, not
     // a lambda: the body exists once per register buffer and the chunk registers never become an addressable array.
     // PACKED: one LOP3 builds the entry (key & R & I) | (R ^ I) with R = ~0xFFF | index bits 4..11 (tile, chunk) and
@@ -740,33 +610,38 @@ __global__ void __launch_bounds__(TC_THREADS, 2) knn_tc_kernel(const __grid_cons
     }                                                                                                                 \
     if (__any_sync(0xffffffffu, cb_addr - cb_addr0 >= flush_bytes)) flush();                                          \
   } while (0)
-    uint32_t va[16], vb[16];
-    __syncwarp();   // tcgen05.ld is warp-collective
-    tmem_ld16_async(tacc, va);
 #pragma unroll 1
-    for (int c16 = 0; c16 < TILE / 16; c16 += 2) {
-      poll_issue();
-      __syncwarp();
-      tmem_wait16(va);
-      tmem_ld16_async(tacc + static_cast<uint32_t>((c16 + 1) * 16), vb);
-      DGCN_TC_FILTER16(va, c16);
-      poll_issue();
-      __syncwarp();
-      tmem_wait16(vb);
-      if (c16 + 2 < TILE / 16) tmem_ld16_async(tacc + static_cast<uint32_t>((c16 + 2) * 16), va);
-      DGCN_TC_FILTER16(vb, c16 + 1);
+    for (int cb = 0; cb < 2; ++cb) {
+      {
+        float d0[32], d1[32];
+        mma_block(cb, d0, d1);
+        __syncthreads();
+        if (cb == 1 && tile + 1 < ntiles && tid == 0) {
+          mbar_expect_tx(&sm.mbar_tma, tile_bytes);
+          tma_planes(stage, (tile + 1) * TILE, &sm.mbar_tma);
+          tma_sx((tile + 1) * TILE, &sm.mbar_tma);
+        }
+        wg_store_m64n64(d0, &sm.acc[0][0], TC_ACC_LD, 0);
+        wg_store_m64n64(d1, &sm.acc[0][0], TC_ACC_LD, 64);
+      }
+      __syncthreads();
+      const float* arow = sm.acc[r];
+#pragma unroll 1
+      for (int c16 = 0; c16 < 4; ++c16) {
+        uint32_t va[16];
+#pragma unroll
+        for (int i = 0; i < 16; i += 4) {
+          const float4 v = *reinterpret_cast<const float4*>(arow + c16 * 16 + i);
+          va[i] = __float_as_uint(v.x); va[i + 1] = __float_as_uint(v.y);
+          va[i + 2] = __float_as_uint(v.z); va[i + 3] = __float_as_uint(v.w);
+        }
+        DGCN_TC_FILTER16(va, cb * 4 + c16);
+      }
     }
 #undef DGCN_TC_FILTER16
-    if (to_issue) {   // (thread 0 only) the filter outran the loads: wait, then issue
-      mbar_wait(&sm.mbar_tma, static_cast<uint32_t>(par));
-      mbar_wait(&sm.mbar_drained, static_cast<uint32_t>(par));
-      issue_tile(tmem + static_cast<uint32_t>((par ^ 1) * TILE));
-    }
   }
   flush();
-  tc_fence_before();
-  __syncthreads();   // every MMA has completed, nobody touches operands or TMEM any more
-  if (warp == 0) tmem_dealloc(sm.tmem_base, 256);
+  __syncthreads();   // every wgmma has completed, nobody touches the operands any more
 
   // ---- exact re-rank of the listed candidates (fp32 FMA chain, k ascending) --------------------------
   uint64_t* list = reinterpret_cast<uint64_t*>(work);   // [KP][TILE]
@@ -796,11 +671,11 @@ __global__ void __launch_bounds__(TC_THREADS, 2) knn_tc_kernel(const __grid_cons
 #pragma unroll 1
       for (int c = 0; c < C; c += 8) {
         float q8[8];
-        ldg256(xqp + c, q8);
+        ldg_f8(xqp + c, q8);
 #pragma unroll
         for (int u = 0; u < KP; ++u) {
           float w[8];
-          ldg256(xtb + off[u] + c, w);
+          ldg_f8(xtb + off[u] + c, w);
 #pragma unroll
           for (int i = 0; i < 8; ++i) dex[u] = fmaf(q8[i], w[i], dex[u]);
         }

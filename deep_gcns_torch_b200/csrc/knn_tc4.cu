@@ -1,4 +1,4 @@
-// knn_tc4_kernel<16 / 28>: the four-tile, warp-specialised tensor-core selection (knn_tc4.cuh) in its own
+// knn_tc4_kernel<16 / 28>: the multi-tile, warp-specialised tensor-core selection (knn_tc4.cuh) in its own
 // translation unit (long ptxas runs of the sorting networks compile in parallel with the other kernels).
 #define DGCN_TEMPLATES_ONLY
 #include "knn_tc4.cuh"

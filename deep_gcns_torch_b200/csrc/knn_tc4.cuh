@@ -1,23 +1,17 @@
-// Four-tile variant of the tensor-core kNN selection (knn_tc.cuh): ONE CTA per SM, warp specialised.
+// Multi-tile variant of the tensor-core kNN selection (knn_tc.cuh): ONE CTA per SM, warp specialised.
 //
-//   Why: knn_tc_kernel is bound by per-warp instruction latency at 8 warps per SM (255 registers, two CTAs whose
-//   TMEM accumulators fill the 512 columns) and 512 query tiles on 296 CTA slots are 1.73 waves.  Here a CTA is
-//   four filter warpgroups (16 warps) + four producer warps; the four warpgroups own four 128-query tiles of the
-//   SAME cloud, so a candidate tile is brought in once (TMA) and multiplied against four resident query operands;
-//   B*N/512 CTAs are a single wave on the 148 SMs for the headline shape.  Registers: launched at 640 x 96,
-//   setmaxnreg moves the producers' share to the filters (512 x 112 + 128 x 32 = the same 61,440).
+//   Why: the CTA holds T4_GROUPS query tiles of the SAME cloud, so a candidate tile is brought in once (TMA) and
+//   multiplied against every resident query operand, and the filter code of knn_tc_kernel is replaced by a cheaper
+//   sorting-network flush.  Two groups: the query planes, the per-group accumulator stage and candidate buffer of a
+//   third would not fit the 227 KB of shared memory an H100 block may use.
 //
-//   producer warp pw         issues the MMAs of warpgroup pw: per half-tile 3*Cpad/16 + 1 tcgen05.mma (M=128, N=64,
-//                            K=16) into one of the group's two 64-column TMEM accumulators (4 x 2 x 64 = all 512
-//                            columns) once the stage has landed (full[s]) and the group has drained that
-//                            accumulator (acc_free[g]); commit -> acc_full[g][h&1] and one arrival on stage_free[s].
-//                            Warp-uniform control flow, one elected lane issues: the descriptors stay in uniform
-//                            registers.  Producer warp 0 also moves the operands by TMA: the query planes of the
-//                            four tiles once, then 64-candidate half-tiles into a two-stage ring (the stage of
-//                            half-tile h+1 is refilled as soon as every group's MMAs of h-1 have completed).
-//   filter warpgroup g       thread r = TMEM lane r = query r of tile g: wait acc_full, tcgen05.ld 8 columns ahead,
-//                            threshold test -> private candidate buffer (shared memory, slot-major); the
-//                            accumulator is handed back (acc_free) as soon as its last chunk sits in registers.
+//   producer warp            moves the operands by TMA: the query planes of the groups once, then 64-candidate
+//                            half-tiles into a two-stage ring (the stage of half-tile h+1 is refilled as soon as every
+//                            group has finished its wgmma on half-tile h-1, stage_free).
+//   filter warpgroup g       per half-tile: wait full[s], two m64n64k16 wgmma chains (query rows 0..63 and 64..127,
+//                            3*Cpad/16 + 1 each) against the stage, release the stage, the accumulators to the group's
+//                            shared-memory stage (row = query); thread r = query r of tile g reads 8 columns at a
+//                            time, threshold test -> private candidate buffer (shared memory, slot-major).
 //                            FLUSH = sorting network instead of one insertion per entry: the batch (<= 16 entries
 //                            per lane, a second pass for slots 16..23) is bitonic-sorted in registers, min-merged
 //                            against the upper half of the 32-entry sorted register list and the list re-sorted by
@@ -39,11 +33,9 @@
 
 namespace dgcn {
 
-constexpr int T4_GROUPS = 4;
-constexpr int T4_THREADS = T4_GROUPS * 128 + 128;                // 4 filter warpgroups + the producer warpgroup (one
-                                                                 // working warp; setmaxnreg moves its registers to the filters)
-constexpr int T4_FILTER_REGS = 112, T4_PRODUCER_REGS = 32;   // 640 x 96 at launch = 512 x 112 + 128 x 32
-constexpr int T4_CT = 64;                                        // candidates per half-tile (UMMA N)
+constexpr int T4_GROUPS = 2;
+constexpr int T4_THREADS = T4_GROUPS * 128 + 32;                 // filter warpgroups + the producer warp
+constexpr int T4_CT = 64;                                        // candidates per half-tile (wgmma N)
 constexpr int T4_STAGES = 2;
 constexpr int T4_CAP = 24;                                       // candidate-buffer slots per thread
 constexpr int T4_FLUSH_AT = 16;                                  // flush when a lane holds this many (checked every 8 candidates)
@@ -52,24 +44,22 @@ constexpr int T4_QBYTES = TC_PLANES * 2 * TC_MAX_C * 128;        // 32 KB: query
 constexpr int T4_STAGE_BYTES = TC_PLANES * TC_MAX_C * 128;       // 16 KB: one 64-candidate half-tile
 constexpr int T4_SX_BYTES = 16 * 128;                            // 2 KB: candidate-side extra K=16 block
 constexpr int T4_CBUF_BYTES = T4_CAP * 128 * 4;                  // 12 KB per group
+constexpr int T4_ACC_LD = 68;                                    // accumulator stage row: 64 columns + 4
+constexpr int T4_ACC_BYTES = TILE * T4_ACC_LD * 4;               // 34 KB per group
 constexpr uint32_t T4_SLOT_STRIDE = 128u * 4u;                   // bytes between two slots of one thread
 static_assert(T4_SLOT_STRIDE == 512u, "the filter's asm bumps the slot pointer by the literal 512");
 
 struct T4Tail {
   uint64_t full[T4_STAGES];               // half-tile operands have landed (TMA complete_tx)
-  uint64_t stage_free[T4_STAGES];         // every MMA reading the stage has completed
-  uint64_t acc_full[T4_GROUPS][2];        // the group's accumulator holds a finished half-tile
-  uint64_t acc_free[T4_GROUPS][2];        // all 128 threads of the group have read it out
+  uint64_t stage_free[T4_STAGES];         // every wgmma reading the stage has completed
   uint64_t q_full;                        // query planes have landed
-  uint32_t tmem_base;
   unsigned char ok[T4_GROUPS][TILE];
 };
 
 constexpr size_t T4_SMEM_BYTES = static_cast<size_t>(T4_GROUPS) * T4_QBYTES + T4_STAGES * (T4_STAGE_BYTES + T4_SX_BYTES) +
-                                 TC_XBLOCK_BYTES + static_cast<size_t>(T4_GROUPS) * T4_CBUF_BYTES + sizeof(T4Tail) + 1024;
-
-constexpr uint32_t kIdescBf16MnMn128x64 =
-    (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((64u >> 3) << 17) | ((128u >> 4) << 24);
+                                 TC_XBLOCK_BYTES + static_cast<size_t>(T4_GROUPS) * (T4_CBUF_BYTES + T4_ACC_BYTES) +
+                                 sizeof(T4Tail) + 1024;
+static_assert(T4_SMEM_BYTES <= 227 * 1024, "one CTA per SM");
 
 // compare-exchange of two register entries (ascending)
 __device__ __forceinline__ void t4_ce(uint32_t& x, uint32_t& y) {
@@ -133,7 +123,8 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
   unsigned char* sx0 = stage0 + T4_STAGES * T4_STAGE_BYTES;                 // [stage][16 rows][128 B]
   unsigned char* qx = sx0 + T4_STAGES * T4_SX_BYTES;                        // ones block, shared by the groups
   unsigned char* cbuf0 = qx + TC_XBLOCK_BYTES;                              // [group][slot][128 threads] u32
-  T4Tail& sm = *reinterpret_cast<T4Tail*>(cbuf0 + T4_GROUPS * T4_CBUF_BYTES);
+  float* acc0 = reinterpret_cast<float*>(cbuf0 + T4_GROUPS * T4_CBUF_BYTES); // [group][128 queries][T4_ACC_LD]
+  T4Tail& sm = *reinterpret_cast<T4Tail*>(reinterpret_cast<unsigned char*>(acc0) + T4_GROUPS * T4_ACC_BYTES);
   const KnnArgs& a = t.a;
   const int tid = threadIdx.x, warp = tid >> 5;
   const int b = blockIdx.y;
@@ -148,13 +139,8 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&t.tm_sqp)) : "memory");
     for (int s = 0; s < T4_STAGES; ++s) {
       mbar_init(&sm.full[s], 1);
-      mbar_init(&sm.stage_free[s], static_cast<uint32_t>(ngroups));
+      mbar_init(&sm.stage_free[s], static_cast<uint32_t>(ngroups * 128));
     }
-    for (int g = 0; g < T4_GROUPS; ++g)
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&sm.acc_full[g][i], 1);
-        mbar_init(&sm.acc_free[g][i], 128);
-      }
     mbar_init(&sm.q_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -169,26 +155,11 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
     reinterpret_cast<uint4*>(sx0)[ch] = make_uint4(0u, 0u, 0u, 0u);
   fence_proxy_async();
   __syncthreads();
-  if (warp == T4_GROUPS * 4) {
-    __syncwarp();
-    tmem_alloc(&sm.tmem_base, 512);     // 4 groups x 2 accumulators x 64 columns
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = sm.tmem_base;
 
   if (warp >= T4_GROUPS * 4) {
-    // ================================ producers ================================
-    // Producer warp pw issues the MMAs of warpgroup pw (tcgen05.commit tracks the issuing thread's own MMAs, so the
-    // four chains are independent); warp 0 of them also moves the operands.  Control flow stays warp-uniform - every
-    // lane waits on the barriers and computes the (uniform) descriptors, one elected lane issues - so that the
-    // descriptors live in uniform registers instead of being rebuilt lane by lane around every tcgen05.mma.
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(T4_PRODUCER_REGS));
-    const int pw = warp - T4_GROUPS * 4;
-    const bool leader = t4_elect_one();
+    // ================================ producer: TMA ================================
     const uint32_t tile_bytes = static_cast<uint32_t>(2 * plane_c + 8 * 128);
-    auto tma_tile = [&](int h) {                           // elected lane of producer warp 0
+    auto tma_tile = [&](int h) {
       const int s = h & 1;
       mbar_expect_tx(&sm.full[s], tile_bytes);
 #pragma unroll
@@ -197,7 +168,7 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
                     (b * TC_PLANES + pl) * Cpad, &sm.full[s]);
       tma_load_2d(smem_u32(sx0 + s * T4_SX_BYTES), &t.tm_sqp, h * T4_CT, b * 8, &sm.full[s]);
     };
-    if (pw == 0 && leader) {
+    if (t4_elect_one()) {
       mbar_expect_tx(&sm.q_full, static_cast<uint32_t>(ngroups * 2 * plane_q));
       for (int g = 0; g < ngroups; ++g)
 #pragma unroll
@@ -207,59 +178,20 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
             tma_load_2d(smem_u32(qbase + g * T4_QBYTES) + pl * plane_q + blk * (Cpad * 128), &t.tm_planes,
                         (qt0 + g) * TILE + blk * 64, (b * TC_PLANES + pl) * Cpad, &sm.q_full);
       tma_tile(0);
-    }
-    __syncwarp();
-    if (pw < ngroups) {
-      const int g = pw;
-      mbar_wait(&sm.q_full, 0u);
-      const uint64_t dqx = umma_desc_mn_sw128(smem_u32(qx), 2048, 1024);
-      const uint32_t abase = smem_u32(qbase + g * T4_QBYTES);
-      const int ksteps = Cpad / 16;
 #pragma unroll 1
-      for (int h = 0; h < H; ++h) {
-        const int s = h & 1;
-        if (pw == 0 && h + 1 < H) {                        // refill the other stage: its MMAs (half-tile h-1) must be done
-          if (h >= 1) mbar_wait_hint(&sm.stage_free[s ^ 1], static_cast<uint32_t>(((h - 1) >> 1) & 1), 1000u);
-          if (leader) tma_tile(h + 1);
-          __syncwarp();
-        }
-        mbar_wait_hint(&sm.full[s], static_cast<uint32_t>((h >> 1) & 1), 1000u);
-        if (h >= 2) mbar_wait_hint(&sm.acc_free[g][s], static_cast<uint32_t>(((h >> 1) - 1) & 1), 1000u);
-        tc_fence_after();
-        const uint32_t bbase = smem_u32(stage0 + s * T4_STAGE_BYTES);
-        const uint64_t dsx = umma_desc_mn_sw128(smem_u32(sx0 + s * T4_SX_BYTES), 2048, 1024);
-        const uint32_t tacc = tmem + static_cast<uint32_t>(g * 128 + s * T4_CT);
-        // descriptors differ only in the start-address field (bits 0..13 = address >> 4)
-        const uint64_t da_hi0 = umma_desc_mn_sw128(abase, Cpad * 128, 1024);
-        const uint64_t da_mid0 = umma_desc_mn_sw128(abase + plane_q, Cpad * 128, 1024);
-        const uint64_t db_hi0 = umma_desc_mn_sw128(bbase, Cpad * 128, 1024);
-        const uint64_t db_mid0 = umma_desc_mn_sw128(bbase + plane_c, Cpad * 128, 1024);
-        if (leader) {
-#pragma unroll 1
-          for (int kk = 0; kk < ksteps; ++kk) {
-            const uint64_t step = static_cast<uint64_t>(kk) * (2048 >> 4);   // (start addresses stay below 2^18: no carry out of the field)
-            // hi*hi, hi*mid, mid*hi  (mid*mid <= 2^-16 |x_i||x_j| is inside eps)
-            umma_bf16(tacc, da_hi0 + step, db_hi0 + step, kIdescBf16MnMn128x64, kk > 0 ? 1u : 0u);
-            umma_bf16(tacc, da_hi0 + step, db_mid0 + step, kIdescBf16MnMn128x64, 1u);
-            umma_bf16(tacc, da_mid0 + step, db_hi0 + step, kIdescBf16MnMn128x64, 1u);
-          }
-          umma_bf16(tacc, dqx, dsx, kIdescBf16MnMn128x64, 1u);   // + 1 x (-|x_j|^2/2)
-          umma_commit(&sm.acc_full[g][s]);
-          umma_commit(&sm.stage_free[s]);                  // one arrival per active group completes the phase
-        }
-        __syncwarp();
+      for (int h = 0; h + 1 < H; ++h) {                    // refill the other stage: its wgmma (half-tile h-1) must be done
+        if (h >= 1) mbar_wait_hint(&sm.stage_free[(h + 1) & 1], static_cast<uint32_t>(((h - 1) >> 1) & 1), 1000u);
+        tma_tile(h + 1);
       }
     }
     __syncwarp();
   } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(T4_FILTER_REGS));
     if ((warp >> 2) < ngroups) {
     // ================================ filter warpgroup ================================
     const int g = warp >> 2;
-    const int r = tid & 127;                               // query row of the tile = TMEM lane
+    const int r = tid & 127;                               // query row of the tile
     const int q0 = (qt0 + g) * TILE, qg = q0 + r;
     const float* sqb = a.sq + static_cast<int64_t>(b) * N;
-    const uint32_t lane_base = static_cast<uint32_t>((warp & 3) * 32) << 16;
     uint32_t lk[T4_LIST];                                  // ascending packed entries (key bits | 12-bit index)
 #pragma unroll
     for (int i = 0; i < T4_LIST; ++i) lk[i] = 0xFFFFFFFFu;
@@ -343,36 +275,67 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
   } while (0)
     // A half-tile is consumed in eight steps of 8 columns, two steps per iteration of a rolled loop (the flush code
     // exists twice plus the final flush, not once per step: the instruction cache matters at ~700 instructions a copy).
+    const uint32_t abase = smem_u32(qbase + g * T4_QBYTES);
+    const uint64_t dqx0 = wg_desc_sw128(smem_u32(qx), 2048, 1024), dqx1 = wg_desc_sw128(smem_u32(qx) + 2048, 2048, 1024);
+    float* accg = acc0 + g * (TILE * T4_ACC_LD);
+    const float* arow = accg + r * T4_ACC_LD;
+    mbar_wait(&sm.q_full, 0u);
 #pragma unroll 1
     for (int h = 0; h < H; ++h) {
-      const int ab = h & 1;
-      mbar_wait(&sm.acc_full[g][ab], static_cast<uint32_t>((h >> 1) & 1));
-      tc_fence_after();
-      const uint32_t tacc = tmem + static_cast<uint32_t>(g * 128 + ab * T4_CT) + lane_base;
-      uint32_t va[8], vb[8];
-      __syncwarp();                                        // tcgen05.ld is warp-collective
-      tmem_ld8_async(tacc, va);
+      const int s = h & 1;
+      mbar_wait_hint(&sm.full[s], static_cast<uint32_t>((h >> 1) & 1), 1000u);
+      {
+        // query rows 0..63 and 64..127 against the 64 staged candidates: hi*hi, hi*mid, mid*hi (mid*mid <= 2^-16
+        // |x_i||x_j| is inside eps), then + 1 x (-|x_j|^2/2)
+        const uint32_t bbase = smem_u32(stage0 + s * T4_STAGE_BYTES);
+        float d0[32], d1[32];
+        wg_fence();
+#pragma unroll 1
+        for (int kk = 0; kk < Cpad / 16; ++kk) {
+          const uint32_t ah = abase + kk * 2048, am = ah + plane_q, bh = bbase + kk * 2048, bm = bh + plane_c;
+          const uint64_t dbh = wg_desc_sw128(bh, Cpad * 128, 1024), dbm = wg_desc_sw128(bm, Cpad * 128, 1024);
+          const uint32_t acc = kk > 0 ? 1u : 0u;
+          wgmma_m64n64<1, 1>(d0, wg_desc_sw128(ah, Cpad * 128, 1024), dbh, acc);
+          wgmma_m64n64<1, 1>(d1, wg_desc_sw128(ah + Cpad * 128, Cpad * 128, 1024), dbh, acc);
+          wgmma_m64n64<1, 1>(d0, wg_desc_sw128(ah, Cpad * 128, 1024), dbm, 1u);
+          wgmma_m64n64<1, 1>(d1, wg_desc_sw128(ah + Cpad * 128, Cpad * 128, 1024), dbm, 1u);
+          wgmma_m64n64<1, 1>(d0, wg_desc_sw128(am, Cpad * 128, 1024), dbh, 1u);
+          wgmma_m64n64<1, 1>(d1, wg_desc_sw128(am + Cpad * 128, Cpad * 128, 1024), dbh, 1u);
+        }
+        const uint64_t dsx = wg_desc_sw128(smem_u32(sx0 + s * T4_SX_BYTES), 2048, 1024);
+        wgmma_m64n64<1, 1>(d0, dqx0, dsx, 1u);
+        wgmma_m64n64<1, 1>(d1, dqx1, dsx, 1u);
+        wg_commit();
+        wg_wait_all();
+        mbar_arrive(&sm.stage_free[s]);                    // my part of the group's reads of the stage is done
+        t4_group_sync(g);                                  // the group has read the previous half-tile out of its stage
+        wg_store_m64n64(d0, accg, T4_ACC_LD, 0);
+        wg_store_m64n64(d1, accg, T4_ACC_LD, 64);
+        t4_group_sync(g);
+      }
+      // eight steps of 8 columns, two per iteration of a rolled loop (the flush code exists twice plus the final
+      // flush, not once per step: the instruction cache matters at ~700 instructions a copy)
 #pragma unroll 1
       for (int c8 = 0; c8 < T4_CT / 8; c8 += 2) {
         // (the warp stays converged through this loop: the flush branch is taken on a warp-wide vote)
         const uint32_t rbits = 0xFFFFF000u | static_cast<uint32_t>(h * T4_CT + c8 * 8);
-        tmem_wait8(va);
-        tmem_ld8_async(tacc + static_cast<uint32_t>((c8 + 1) * 8), vb);
-        DGCN_T4_FILTER8(va, rbits);
-        tmem_wait8(vb);
-        if (c8 + 2 < T4_CT / 8) {
-          tmem_ld8_async(tacc + static_cast<uint32_t>((c8 + 2) * 8), va);
-        } else {
-          tc_fence_before();                               // the whole accumulator sits in registers: hand it back
-          mbar_arrive(&sm.acc_free[g][ab]);
+        uint32_t va[8], vb[8];
+        {
+          const float4 u0 = *reinterpret_cast<const float4*>(arow + c8 * 8), u1 = *reinterpret_cast<const float4*>(arow + c8 * 8 + 4);
+          const float4 w0 = *reinterpret_cast<const float4*>(arow + c8 * 8 + 8), w1 = *reinterpret_cast<const float4*>(arow + c8 * 8 + 12);
+          va[0] = __float_as_uint(u0.x); va[1] = __float_as_uint(u0.y); va[2] = __float_as_uint(u0.z); va[3] = __float_as_uint(u0.w);
+          va[4] = __float_as_uint(u1.x); va[5] = __float_as_uint(u1.y); va[6] = __float_as_uint(u1.z); va[7] = __float_as_uint(u1.w);
+          vb[0] = __float_as_uint(w0.x); vb[1] = __float_as_uint(w0.y); vb[2] = __float_as_uint(w0.z); vb[3] = __float_as_uint(w0.w);
+          vb[4] = __float_as_uint(w1.x); vb[5] = __float_as_uint(w1.y); vb[6] = __float_as_uint(w1.z); vb[7] = __float_as_uint(w1.w);
         }
+        DGCN_T4_FILTER8(va, rbits);
         DGCN_T4_FILTER8(vb, rbits + 8u);
       }
     }
 #undef DGCN_T4_FILTER8
     flush();
-    t4_group_sync(g);   // the group's MMAs have completed (every thread saw the last acc_full) and nobody of the
-                        // group flushes any more: its query planes and candidate buffer become the work area
+    t4_group_sync(g);   // the group's wgmma have completed and nobody of the group flushes any more: its query
+                        // planes and candidate buffer become the work area
 
     const float cut = (lk[KP - 1] == 0xFFFFFFFFu) ? INFINITY : __uint_as_float(lk[KP - 1] & 0xFFFFF000u);
     const int C = a.C;
@@ -448,11 +411,11 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
 #pragma unroll 1
         for (int c = 0; c < C; c += 8) {
           float q8[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-          if (m0 < nbe) ldg256(xqp + c, q8);
+          if (m0 < nbe) ldg_f8(xqp + c, q8);
 #pragma unroll
           for (int i4 = 0; i4 < 4; ++i4) {
             float w[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-            if (m0 + i4 < nbe) ldg256(xtb + jj[i4] * static_cast<uint32_t>(C) + c, w);
+            if (m0 + i4 < nbe) ldg_f8(xtb + jj[i4] * static_cast<uint32_t>(C) + c, w);
 #pragma unroll
             for (int i = 0; i < 8; ++i) dot[i4] = fmaf(q8[i], w[i], dot[i4]);
           }
@@ -482,7 +445,7 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
     // ---- exact re-rank of the listed candidates (fp32 FMA chain, channels ascending) --------------------------
     uint64_t* list = reinterpret_cast<uint64_t*>(qbase + g * T4_QBYTES);   // [KP][TILE]
     {
-      // Two halves of KP/2 candidates (register budget of a 17-warp CTA).  Channels in chunks of 8 in the outer
+      // Two halves of KP/2 candidates (register budget of a 9-warp CTA at one CTA per SM).  Channels in chunks of 8 in the outer
       // loop, candidates in the inner one: KP/2 independent FMA chains in flight; per candidate the chain is
       // acc = fma(x_q[c], x_j[c], acc) for c ascending from acc = 0 - the bits of the fp32 kernel.
       constexpr int HN = KP / 2;
@@ -495,13 +458,13 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
 #pragma unroll 1
         for (int c = 0; c < C; c += 8) {
           float q8[8];
-          ldg256(xqp + c, q8);
+          ldg_f8(xqp + c, q8);
 #pragma unroll
           for (int u = 0; u < HN; ++u) {
             const uint32_t en = lk[half * HN + u];
             const uint32_t j = en != 0xFFFFFFFFu ? (en & 0xFFFu) : static_cast<uint32_t>(qg);
             float w[8];
-            ldg256(xtb + j * static_cast<uint32_t>(C) + c, w);
+            ldg_f8(xtb + j * static_cast<uint32_t>(C) + c, w);
 #pragma unroll
             for (int i = 0; i < 8; ++i) dex[u] = fmaf(q8[i], w[i], dex[u]);
           }
@@ -549,9 +512,6 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
     }
     }
   }
-  tc_fence_before();
-  __syncthreads();   // every MMA has completed and every accumulator has been read
-  if (warp == T4_GROUPS * 4) tmem_dealloc(tmem, 512);
 }
 
 inline bool knn_tc4_list_ok(int kp, int k) {

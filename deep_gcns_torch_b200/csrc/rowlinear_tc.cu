@@ -1,31 +1,31 @@
-// Row-wise Linear with fused bias / skip connection on the tcgen05 tensor cores:
+// Row-wise Linear with fused bias / skip connection on the Hopper tensor cores (wgmma):
 //
 //     out[n][m] = sum_k a[n][k] * W[m][k]  (+ bias[m])  (+ res[n][m])          a (N,K), W (M,K), out / res (N,M), fp32
 //
 // = the `Linear` that ends GENConv's MLP (gcn_lib/sparse/torch_nn.py:56-68, mlp_layers = 1) together with the
-// `+ h` of DeeperGCN's 'res+' block (examples/ogb/ogbn_arxiv/model.py:91-106): north_star's "tensor cores for
-// the MLP GEMM".  The GEMM is skinny (K, M <= 256) and the rows are many, so it is bound by HBM (read a and res,
-// write out once each), not by the tensor pipe; the point of the kernel is that everything else rides on that
-// single pass.
+// `+ h` of DeeperGCN's 'res+' block (examples/ogb/ogbn_arxiv/model.py:91-106).  The GEMM is skinny (K, M <= 256)
+// and the rows are many, so it is bound by HBM (read a and res, write out once each), not by the tensor pipe; the
+// point of the kernel is that everything else rides on that single pass.
 //
 // fp32 accuracy on bf16 tensor cores: a = a_hi + a_mid, W = W_hi + W_mid (bf16 round-to-nearest each,
-// |x - hi - mid| <= 2^-17 |x|), products a_hi W_hi + a_hi W_mid + a_mid W_hi + a_mid W_mid accumulated in fp32 in
-// TMEM: error <= ~2^-16 sum_k |a||W| (1.5e-5 relative to the magnitude sum), two orders below the 1e-3 parity
+// |x - hi - mid| <= 2^-17 |x|), products a_hi W_hi + a_hi W_mid + a_mid W_hi + a_mid W_mid accumulated in fp32:
+// error <= ~2^-16 sum_k |a||W| (1.5e-5 relative to the magnitude sum), two orders below the 1e-3 parity
 // tolerance.  W is split once per call by a prep kernel; a is split on the fly by the producer warps.
 //
 // One persistent CTA per SM, 384 threads:
-//   warps 8-11 (producers)  tile of 128 rows: coalesced 256-bit loads of a -> (hi, mid) bf16 -> shared memory in the
-//                          canonical K-major SWIZZLE_128B UMMA layout [plane][K/64][128 rows][128 B]; the first
-//                          producer thread then issues the 4 x K/16 tcgen05.mma (M=128, N=M_out, K=16) into one of
-//                          two TMEM accumulators and commits.
-//   warps 0-7 (epilogue)   previous tile, two warps per TMEM lane quarter taking alternate 32-column blocks (twice the
-//                          skip-connection loads in flight): tcgen05.ld (thread = row, 32 columns), transpose through a padded
-//                          shared-memory stage, then row-contiguous out = acc + bias + res.
+//   warps 8-11 (producers)  tile of 128 rows: coalesced 128-bit loads of a -> (hi, mid) bf16 -> shared memory in the
+//                          canonical K-major SWIZZLE_128B layout [plane][K/64][128 rows][128 B].
+//   warps 0-7 (consumers)  warpgroup wg = rows 64 wg .. 64 wg + 63 of the tile: 4 x K/16 wgmma m64n32k16 per 32-column
+//                          block of the output into registers (up to 8 blocks = M 256), the A buffer is handed back to
+//                          the producers as soon as the wgmma have completed - they fill the next tile under this
+//                          epilogue -, then out = acc + bias + res straight from the accumulator fragments (each quad
+//                          of lanes covers 8 consecutive floats = one 32-byte sector of a row).
 //   W (hi, mid)            resident in shared memory for the life of the CTA, loaded once by TMA.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace dgcn {
 
@@ -65,44 +65,6 @@ __device__ __forceinline__ void rl_tma_load_2d(uint32_t smem_dst, const CUtensor
       "l"(reinterpret_cast<uint64_t>(map)), "r"(rl_smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-// K-major operand, SWIZZLE_128B: rows of 64 bf16 (128 B), 8-row groups 1024 B apart (cute::UMMA::SmemDescriptor)
-__device__ __forceinline__ uint64_t rl_desc_k_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu);
-  d |= static_cast<uint64_t>(1) << 16;                         // leading-dim offset: unused with swizzled K-major
-  d |= static_cast<uint64_t>((1024u >> 4) & 0x3FFFu) << 32;    // stride between 8-row groups
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;                         // SWIZZLE_128B
-  return d;
-}
-__device__ __forceinline__ void rl_umma(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void rl_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(rl_smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void rl_tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
 // W (M,K) fp32 -> Wp (2, M, K) bf16 (hi, mid)
 __global__ void rl_split_weights_kernel(const float* __restrict__ w, int64_t n, __nv_bfloat16* __restrict__ wp) {
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -121,18 +83,16 @@ struct RlArgs {
   float* out;
   int64_t N;
   int K, M;
-  int tmem_cols;            // 2 accumulators of M columns, rounded to a power of two >= 32
 };
 
 struct RlBars {
   uint64_t w_full;          // W planes landed
   uint64_t a_full;          // all 128 producer threads wrote (and fenced) their part of the A tile
-  uint64_t mma_done[2];     // MMAs of the tile in accumulator i have completed (A free, accumulator readable)
-  uint64_t acc_free[2];     // the 256 epilogue threads have drained accumulator i
-  uint32_t tmem_base;
+  uint64_t a_free;          // the 256 consumer threads' wgmma on the A tile have completed
 };
 
 constexpr int RL_EPI_THREADS = 256;   // warps 0..7
+constexpr int RL_NB = RL_MAX / 32;    // 32-column output blocks
 
 __global__ void __launch_bounds__(RL_EPI_THREADS + 128, 1) rowlinear_tc_kernel(const __grid_constant__ RlArgs g) {
   extern __shared__ __align__(16) unsigned char rl_smem[];
@@ -143,33 +103,20 @@ __global__ void __launch_bounds__(RL_EPI_THREADS + 128, 1) rowlinear_tc_kernel(c
   const uint32_t a_plane = static_cast<uint32_t>(RL_TILE) * K * 2;
   unsigned char* w_s = base;                                            // [2][kblocks][M][128 B]
   unsigned char* a_s = w_s + 2 * w_plane;                               // [2][kblocks][128][128 B]
-  float* stage = reinterpret_cast<float*>(a_s + 2 * a_plane);           // [8 warps][32][33]
-  RlBars& bar = *reinterpret_cast<RlBars*>(reinterpret_cast<unsigned char*>(stage) + 8 * 32 * 33 * 4);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  RlBars& bar = *reinterpret_cast<RlBars*>(a_s + 2 * a_plane);
+  const int tid = threadIdx.x, warp = tid >> 5;
   const int64_t ntiles = (g.N + RL_TILE - 1) / RL_TILE;
 
   if (tid == 0) {
     rl_mbar_init(&bar.w_full, 1);
     rl_mbar_init(&bar.a_full, 128);
-    rl_mbar_init(&bar.mma_done[0], 1);
-    rl_mbar_init(&bar.mma_done[1], 1);
-    rl_mbar_init(&bar.acc_free[0], RL_EPI_THREADS);
-    rl_mbar_init(&bar.acc_free[1], RL_EPI_THREADS);
+    rl_mbar_init(&bar.a_free, RL_EPI_THREADS);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(rl_smem_u32(&bar.tmem_base)),
-                 "r"(static_cast<uint32_t>(g.tmem_cols))
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = bar.tmem_base;
 
   if (warp >= RL_EPI_THREADS / 32) {
-    // ======================= producers (+ MMA issue by their first thread) ===========================================
+    // ======================= producers ===============================================================================
     const int pt = tid - RL_EPI_THREADS;
     if (pt == 0) {   // W: one box of 64 k x M rows per (plane, k-block)
       rl_mbar_expect_tx(&bar.w_full, 2 * w_plane);
@@ -177,15 +124,12 @@ __global__ void __launch_bounds__(RL_EPI_THREADS + 128, 1) rowlinear_tc_kernel(c
         for (int kb = 0; kb < kblocks; ++kb)
           rl_tma_load_2d(rl_smem_u32(w_s) + pl * w_plane + kb * (M * 128), &g.tm_w, kb * 64, pl * M, &bar.w_full);
     }
-    // instruction descriptor: D fp32, A / B bf16, both K-major, N = M_out, M = 128
-    const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((static_cast<uint32_t>(M) >> 3) << 17) | ((128u >> 4) << 24);
     const int chunks = K / 8;                       // 16-byte bf16 chunks per row
     const int rows_per_pass = 128 / chunks;         // K = 64: 16 rows, 128: 8 rows, 256: 4 rows
     const int cg = pt % chunks, rsub = pt / chunks; // my chunk of the row, my row inside a pass
     const int kb = cg >> 3, c = cg & 7;
     int64_t it = 0;
     for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const int acc = static_cast<int>(it & 1);
       const int64_t row0 = tile * RL_TILE;
       // eight passes at a time: all sixteen 128-bit loads of a group are issued before the first conversion, so a
       // producer warp keeps 8 KB of the a-stream in flight (the kernel is HBM bound: memory-level parallelism is
@@ -203,8 +147,8 @@ __global__ void __launch_bounds__(RL_EPI_THREADS + 128, 1) rowlinear_tc_kernel(c
             hi4[p8] = __ldg(src + 1);
           }
         }
-        // the A buffer is still read by the previous tile's MMAs: wait only now, with this tile's first loads in flight
-        if (r0 == 0 && it > 0) rl_mbar_wait(&bar.mma_done[acc ^ 1], static_cast<uint32_t>(((it - 1) >> 1) & 1));
+        // the A buffer is still read by the previous tile's wgmma: wait only now, with this tile's first loads in flight
+        if (r0 == 0 && it > 0) rl_mbar_wait(&bar.a_free, static_cast<uint32_t>((it - 1) & 1));
 #pragma unroll
         for (int p8 = 0; p8 < 8; ++p8) {
           const int row = r0 + p8 * rows_per_pass + rsub;
@@ -226,73 +170,64 @@ __global__ void __launch_bounds__(RL_EPI_THREADS + 128, 1) rowlinear_tc_kernel(c
       }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");       // my generic-proxy stores -> tensor-core reads
       rl_mbar_arrive(&bar.a_full);
-      if (pt == 0) {
-        if (it == 0) rl_mbar_wait(&bar.w_full, 0u);
-        rl_mbar_wait(&bar.a_full, static_cast<uint32_t>(it & 1));
-        if (it >= 2) rl_mbar_wait(&bar.acc_free[acc], static_cast<uint32_t>(((it - 2) >> 1) & 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t d = tmem + static_cast<uint32_t>(acc * M);
-        uint32_t accum = 0;
-        for (int kk = 0; kk < K / 16; ++kk) {
-          const uint32_t koff = static_cast<uint32_t>(kk >> 2) * (RL_TILE * 128) + static_cast<uint32_t>(kk & 3) * 32;
-          const uint32_t woff = static_cast<uint32_t>(kk >> 2) * (M * 128) + static_cast<uint32_t>(kk & 3) * 32;
-#pragma unroll
-          for (int term = 0; term < 4; ++term) {   // hi*hi, hi*mid, mid*hi, mid*mid
-            const uint32_t pa = (term >> 1) * a_plane, pb = (term & 1) * w_plane;
-            rl_umma(d, rl_desc_k_sw128(rl_smem_u32(a_s) + pa + koff), rl_desc_k_sw128(rl_smem_u32(w_s) + pb + woff), idesc,
-                    accum);
-            accum = 1;
-          }
-        }
-        rl_commit(&bar.mma_done[acc]);
-      }
     }
   } else {
-    // ======================= epilogue: out = acc + bias + res ========================================================
-    float* st = stage + warp * 32 * 33;
-    const int quarter = warp & 3, half = warp >> 2;      // TMEM lane quarter; which of the alternating column blocks
+    // ======================= consumers: wgmma, then out = acc + bias + res ==========================================
+    const int wg = warp >> 2;
+    const int nb = M / 32;
+    const uint32_t a_base = rl_smem_u32(a_s) + static_cast<uint32_t>(wg) * (64 * 128);   // rows 64 wg .. of every k-block
+    const uint32_t w_base = rl_smem_u32(w_s);
     int64_t it = 0;
     for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const int acc = static_cast<int>(it & 1);
-      rl_mbar_wait(&bar.mma_done[acc], static_cast<uint32_t>((it >> 1) & 1));
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int64_t row0 = tile * RL_TILE + quarter * 32;
-      // lane = column.  The 32 rows' skip-connection values of a 32-column block are loaded one block ahead: 32
-      // independent 128-byte row segments per warp stay in flight while the previous block is read from TMEM,
-      // transposed through the padded stage and stored.
-      float rv[32], rn[32];
+      if (it == 0) rl_mbar_wait(&bar.w_full, 0u);
+      rl_mbar_wait(&bar.a_full, static_cast<uint32_t>(it & 1));
+      float d[RL_NB][16];
+      wg_fence();
 #pragma unroll
-      for (int rr = 0; rr < 32; ++rr)
-        rv[rr] = (g.res && half * 32 < M && row0 + rr < g.N) ? __ldg(g.res + (row0 + rr) * M + half * 32 + lane) : 0.f;
-      for (int cb = half * 32; cb < M; cb += 64) {
-        const bool more = cb + 64 < M;
+      for (int j = 0; j < RL_NB; ++j) {
+        if (j < nb) {
+          for (int kk = 0; kk < K / 16; ++kk) {
+            const uint32_t koff = static_cast<uint32_t>(kk >> 2) * (RL_TILE * 128) + static_cast<uint32_t>(kk & 3) * 32;
+            const uint32_t woff = static_cast<uint32_t>(kk >> 2) * (M * 128) + static_cast<uint32_t>(j) * (32 * 128) +
+                                  static_cast<uint32_t>(kk & 3) * 32;
 #pragma unroll
-        for (int rr = 0; rr < 32; ++rr)
-          rn[rr] = (more && g.res && row0 + rr < g.N) ? __ldg(g.res + (row0 + rr) * M + cb + 64 + lane) : 0.f;
-        uint32_t v[32];
-        __syncwarp();
-        rl_tmem_ld32(tmem + static_cast<uint32_t>(acc * M + cb) + (static_cast<uint32_t>(quarter * 32) << 16), v);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) st[lane * 33 + j] = __uint_as_float(v[j]);
-        __syncwarp();
-        const float bv = g.bias ? __ldg(g.bias + cb + lane) : 0.f;
-#pragma unroll
-        for (int rr = 0; rr < 32; ++rr) {
-          const int64_t row = row0 + rr;
-          if (row < g.N) g.out[row * M + cb + lane] = (st[rr * 33 + lane] + bv) + rv[rr];
+            for (int term = 0; term < 4; ++term) {   // hi*hi, hi*mid, mid*hi, mid*mid
+              const uint32_t pa = (term >> 1) * a_plane, pb = (term & 1) * w_plane;
+              wgmma_m64n32<0, 0>(d[j], wg_desc_sw128(a_base + pa + koff, 16, 1024), wg_desc_sw128(w_base + pb + woff, 16, 1024),
+                                 (kk | term) != 0 ? 1u : 0u);
+            }
+          }
         }
-#pragma unroll
-        for (int rr = 0; rr < 32; ++rr) rv[rr] = rn[rr];
       }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      rl_mbar_arrive(&bar.acc_free[acc]);
+      wg_commit();
+      wg_wait_all();
+      rl_mbar_arrive(&bar.a_free);
+      const int64_t rbase = tile * RL_TILE + wg * 64;
+#pragma unroll
+      for (int j = 0; j < RL_NB; ++j) {
+        if (j < nb) {
+#pragma unroll
+          for (int i = 0; i < 16; i += 2) {
+            const int64_t row = rbase + wg_frag_row(i);
+            const int col = j * 32 + wg_frag_col(i);
+            if (row < g.N) {
+              float2 v = make_float2(d[j][i], d[j][i + 1]);
+              if (g.bias) {   // two scalar loads: bias needs only 4-byte alignment (M floats, L1-resident)
+                v.x += __ldg(g.bias + col);
+                v.y += __ldg(g.bias + col + 1);
+              }
+              if (g.res) {
+                const float2 rv = __ldg(reinterpret_cast<const float2*>(g.res + row * M + col));
+                v.x += rv.x;
+                v.y += rv.y;
+              }
+              *reinterpret_cast<float2*>(g.out + row * M + col) = v;
+            }
+          }
+        }
+      }
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(static_cast<uint32_t>(g.tmem_cols))
-                 : "memory");
 }
 
 typedef CUresult (*RlEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -312,10 +247,10 @@ static RlEncodeFn rl_encoder() {
 }
 
 static size_t rl_smem_bytes(int64_t K, int64_t M) {
-  return static_cast<size_t>(2) * M * K * 2 + static_cast<size_t>(2) * RL_TILE * K * 2 + 8 * 32 * 33 * 4 + sizeof(RlBars) + 1024;
+  return static_cast<size_t>(2) * M * K * 2 + static_cast<size_t>(2) * RL_TILE * K * 2 + sizeof(RlBars) + 1024;
 }
 static bool rl_shape_ok(int64_t K, int64_t M) {
-  // 128 | rows per pass = 1024 / K; W planes + A planes + stage must fit the 227 KB of one SM
+  // 128 | rows per pass = 1024 / K; W planes + A planes must fit the 227 KB of one SM
   return (K == 64 || K == 128 || K == 256) && M >= 32 && M <= RL_MAX && M % 32 == 0 && rl_smem_bytes(K, M) <= 227 * 1024;
 }
 
@@ -355,12 +290,9 @@ int dgcn_linear_residual(const float* a, int64_t N, int64_t K, const float* weig
       return DGCN_ERR_CUDA;
   }
   g.a = a; g.bias = bias; g.res = res; g.out = out; g.N = N; g.K = static_cast<int>(K); g.M = static_cast<int>(M);
-  int cols = 32;
-  while (cols < 2 * M) cols <<= 1;
-  g.tmem_cols = cols;
   const size_t smem = rl_smem_bytes(K, M);
   DGCN_ENSURE_SMEM((rowlinear_tc_kernel), smem);
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 0;
   DGCN_CUDA_TRY(cudaGetDevice(&dev));
   DGCN_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const int64_t ntiles = ceil_div(N, RL_TILE);

@@ -339,7 +339,7 @@ static int launch_aggr(const AggrArgs& g, cudaStream_t stream) {
   case A:                                                                                   \
     if (grid) genconv_aggregate_kernel<VEC, NBLK, A, 0, PRE><<<grid, warps * 32, 0, stream>>>(g); \
     if (g.hub_rows && g.run_hubs) {                                                                     \
-      genconv_aggregate_kernel<VEC, NBLK, A, 1, PRE><<<592, 256, 0, stream>>>(g);                \
+      genconv_aggregate_kernel<VEC, NBLK, A, 1, PRE><<<4 * device_sm_count(), 256, 0, stream>>>(g); \
       genconv_aggregate_kernel<VEC, NBLK, A, 2, PRE><<<32, 256, 0, stream>>>(g);                 \
     }                                                                                       \
     break;

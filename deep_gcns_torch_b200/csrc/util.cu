@@ -14,6 +14,32 @@ void set_last_cuda_error(cudaError_t e, const char* file, int line) {
   (void)cudaGetLastError();   // reported through the status code: do not leave it for an unrelated later launch check
 }
 
+static int device_attr(cudaDeviceAttr attr, std::atomic<int>* cache, int fallback) {
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return fallback;
+  int v = cache[dev].load(std::memory_order_relaxed);
+  if (v > 0) return v;
+  if (cudaDeviceGetAttribute(&v, attr, dev) != cudaSuccess || v <= 0) return fallback;
+  cache[dev].store(v, std::memory_order_relaxed);
+  return v;
+}
+int device_sm_count() {
+  static std::atomic<int> cache[64];
+  return device_attr(cudaDevAttrMultiProcessorCount, cache, 132);
+}
+size_t device_l2_bytes() {
+  static std::atomic<int> cache[64];
+  return static_cast<size_t>(device_attr(cudaDevAttrL2CacheSize, cache, 50 << 20));
+}
+
+static std::atomic<int> g_cert_on{0};
+static std::atomic<int64_t> g_cert_failed{0}, g_cert_queries{0};
+bool debug_certification_on() { return g_cert_on.load(std::memory_order_relaxed) != 0; }
+void debug_certification_add(int64_t uncertified, int64_t queries) {
+  g_cert_failed.fetch_add(uncertified, std::memory_order_relaxed);
+  g_cert_queries.fetch_add(queries, std::memory_order_relaxed);
+}
+
 struct TimedLaunch {
   std::string tag;
   cudaEvent_t beg, end;
@@ -71,12 +97,21 @@ int dgcn_debug_kernel_timing_read(const char* tag, double* total_ms, int64_t* la
   *launches = n;
   return DGCN_OK;
 }
+int dgcn_debug_tc_certification(int32_t enable) {
+  return dgcn::g_cert_on.exchange(enable ? 1 : 0);
+}
+int dgcn_debug_tc_certification_read(int64_t* uncertified, int64_t* queries) {
+  if (!uncertified || !queries) return DGCN_ERR_BAD_ARG;
+  *uncertified = dgcn::g_cert_failed.exchange(0);
+  *queries = dgcn::g_cert_queries.exchange(0);
+  return DGCN_OK;
+}
 int dgcn_version(void) { return 100; }
 const char* dgcn_status_string(int status) {
   switch (status) {
     case DGCN_OK: return "ok";
     case DGCN_ERR_BAD_ARG: return "bad argument (null pointer or inconsistent size)";
-    case DGCN_ERR_UNSUPPORTED: return "request outside what the sm_100a kernels cover";
+    case DGCN_ERR_UNSUPPORTED: return "request outside what the sm_90a kernels cover";
     case DGCN_ERR_WORKSPACE: return "workspace too small";
     case DGCN_ERR_CUDA: return "CUDA launch failed";
     default: return "unknown status";

@@ -1,3 +1,3 @@
 """Drop-in for the reference's `gcn_lib` package (same sub-packages, class names,
 constructor / forward signatures and state_dict keys; SURVEY.md 8b), with the
-message-passing arithmetic running in the sm_100a kernels of libdgcn.so."""
+message-passing arithmetic running in the sm_90a kernels of libdgcn.so."""

@@ -9,8 +9,8 @@ mlp_layers=1 ends in one Linear.  `res_plus_block` runs the same arithmetic in t
 
     dgcn_genconv_aggregate_fused   reads h rows as relu(s*h + t) (gathered rows and the residual row),
                                    message + aggregate + MsgNorm + (z_i + m_i)     -> a
-    dgcn_linear_residual           h_out = h + a W^T + b on the tcgen05 tensor cores (two-plane bf16 split of both
-                                   operands, fp32 accumulation in TMEM; bias and skip connection in the epilogue)
+    dgcn_linear_residual           h_out = h + a W^T + b on the tensor cores (wgmma; two-plane bf16 split of both
+                                   operands, fp32 accumulation; bias and skip connection in the epilogue)
 
 so the normalised / activated copy of h and the GENConv output before the skip connection are never
 written to HBM (three N x C passes fewer per layer).  A model opts in by replacing the four lines above
@@ -64,7 +64,7 @@ def _prm(conv):
 
 
 def _linear_plus(lin, a, h, out=None):
-    """h + a W^T + b: the tcgen05 row-Linear with bias and skip connection in its epilogue (one pass over a, h and
+    """h + a W^T + b: the tensor-core row-Linear with bias and skip connection in its epilogue (one pass over a, h and
     the result); shapes it does not cover keep cuBLAS with the skip connection riding on the GEMM's beta."""
     if a.is_cuda and _native.linear_residual_supported(lin.in_features, lin.out_features) and \
             a.data_ptr() % 16 == 0 and h.data_ptr() % 16 == 0 and (out is None or out.data_ptr() % 16 == 0):

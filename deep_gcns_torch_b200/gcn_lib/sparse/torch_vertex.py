@@ -43,7 +43,7 @@ class GENConv(GenMessagePassing):
         scale = self.msg_norm.msg_scale if self.msg_norm is not None else None
         h = self.propagate(edge_index, x=x, edge_attr=edge_emb, msg_scale=scale, residual=True)
         if not torch.is_grad_enabled() and len(self.mlp) == 1 and isinstance(self.mlp[0], nn.Linear):
-            lin = self.mlp[0]                      # inference, mlp_layers = 1: the Linear on the tcgen05 tensor cores
+            lin = self.mlp[0]                      # inference, mlp_layers = 1: the Linear on the tensor cores
             if _native.linear_residual_supported(lin.in_features, lin.out_features) and h.data_ptr() % 16 == 0:
                 return _native.linear_residual(h, lin.weight, lin.bias)
         return self.mlp(h)

@@ -1,5 +1,5 @@
 /*
- * dgcn.h - C ABI of the B200-native message-passing hot path of deep_gcns_torch.
+ * dgcn.h - C ABI of the H100-native message-passing hot path of deep_gcns_torch.
  *
  * The reference (lightaime/deep_gcns_torch) has no FFI / plugin layer: its
  * boundary is the Python nn.Module API (SURVEY.md 8b).  This header is the
@@ -16,7 +16,7 @@
  *     allocates: scratch memory is a caller-owned workspace sized by the
  *     matching *_workspace_bytes() query;
  *   - return value: DGCN_OK or a negative dgcn_status; no exceptions cross.
- *   - kernels are compiled for sm_100a only.
+ *   - kernels are compiled for sm_90a (H100) only.
  */
 #ifndef DGCN_H_
 #define DGCN_H_
@@ -92,13 +92,13 @@ typedef struct dgcn_basic_conv {
  * array drawn by the caller from the CPU generator, torch_edge.py:22-24). */
 /* flags: DGCN_KNN_EXACT_FP32 ranks with the fp32 FMA kernels only (no tensor-core
  * pre-filter); DGCN_KNN_TC_TILE_PER_CTA keeps the tensor-core pre-filter on the
- * one-tile-per-CTA kernel where the four-tile warp-specialised kernel would be chosen.
+ * one-tile-per-CTA kernel where the multi-tile warp-specialised kernel would be chosen.
  * The result is the same list either way - the switches exist for A/B tests and
  * measurements and are a property of the CALL, not of the process. */
 enum dgcn_knn_flags {
   DGCN_KNN_DEFAULT = 0,
   DGCN_KNN_EXACT_FP32 = 1,
-  DGCN_KNN_TC_TILE_PER_CTA = 2 /* tensor-core path: always the one-tile-per-CTA kernel, never the four-tile one */
+  DGCN_KNN_TC_TILE_PER_CTA = 2 /* tensor-core path: always the one-tile-per-CTA kernel, never the multi-tile one */
 };
 typedef struct dgcn_dilation {
   int64_t k;
@@ -276,12 +276,12 @@ int dgcn_genconv_aggregate_fused(const float* x_src, const float* x_dst, int64_t
                                  const dgcn_genconv_fusion* fus /* may be NULL */, float* out,
                                  dgcn_stream_t stream);
 
-/* Row-wise Linear with fused bias and skip connection on the tcgen05 tensor cores:
+/* Row-wise Linear with fused bias and skip connection on the tensor cores (wgmma):
  *   out[n][m] = sum_k a[n][k] * weight[m][k] (+ bias[m]) (+ res[n][m])
  * = the Linear that ends GENConv's MLP (gcn_lib/sparse/torch_nn.py:56-68 with mlp_layers = 1; nn.Linear
  * weight layout (M, K)) plus the `+ h` of DeeperGCN's res+ block (examples/ogb/ogbn_arxiv/model.py:104).
  * fp32 in / out; the product runs as a two-plane bf16 split of both operands (4 tensor-core products, fp32
- * accumulation in TMEM, error <= ~2^-16 * sum_k |a||w|).  K in {64, 128, 256}, M a multiple of 32 up to 256,
+ * accumulation, error <= ~2^-16 * sum_k |a||w|).  K in {64, 128, 256}, M a multiple of 32 up to 256,
  * 16-byte aligned rows; anything else returns DGCN_ERR_UNSUPPORTED (callers keep cuBLAS for those).
  * bias, res may be NULL; out may alias res.  ws: dgcn_linear_residual_workspace_bytes(K, M) (0 = unsupported). */
 size_t dgcn_linear_residual_workspace_bytes(int64_t K, int64_t M);
@@ -317,6 +317,14 @@ int dgcn_gather_rows(const float* x, int64_t C, const int32_t* rows, int64_t R, 
  * --------------------------------------------------------------------- */
 int dgcn_debug_kernel_timing(int32_t enable);
 int dgcn_debug_kernel_timing_read(const char* tag, double* total_ms, int64_t* launches);
+
+/* Measurement hook (tests): when enabled, every call that takes the tensor-core
+ * kNN pre-filter synchronises its stream after the selection and adds the
+ * number of queries the pre-filter could not certify (they were completed by
+ * the exact fp32 kernel) and the number of queries to two counters.  _read()
+ * returns and resets them.  Off by default: the synchronisation costs time. */
+int dgcn_debug_tc_certification(int32_t enable);
+int dgcn_debug_tc_certification_read(int64_t* uncertified, int64_t* queries);
 
 #ifdef __cplusplus
 }

@@ -10,8 +10,8 @@ reference on the same host; the fp64 flavour adjudicates fp32 near-ties.
 
 Pinned by tests/test_oracle_pins.py against (a) the golden vectors under
 tests/golden/ that tests/golden/gen_golden.py produced by running the
-UNMODIFIED reference modules (oracle/ref_shims.py), and (b) the live reference
-whenever /root/reference is present.
+UNMODIFIED reference modules (oracle/ref_shims.py), and (b) the reference's
+outputs on random shapes stored the same way (ref_random_shapes.npz).
 """
 import torch
 import torch.nn.functional as F

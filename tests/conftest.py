@@ -9,14 +9,14 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):
     import torch
     if torch.cuda.is_available():
         return
-    skip = pytest.mark.skip(reason="no CUDA device in this container")
+    skip = pytest.mark.skip(reason="no CUDA device")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

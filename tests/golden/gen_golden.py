@@ -1,9 +1,9 @@
 """Generates the committed golden vectors under tests/golden/*.npz by running
-the UNMODIFIED reference modules (/root/reference/gcn_lib, loaded through
+the UNMODIFIED reference modules (gcn_lib of a reference checkout, loaded through
 oracle/ref_shims.py) on seeded synthetic inputs.  The reference has no tests
 or fixtures of its own (SURVEY.md 4), so these vectors are what pins parity.
 
-    python tests/golden/gen_golden.py        # needs /root/reference
+    DGCN_REFERENCE_ROOT=<reference checkout> python tests/golden/gen_golden.py
 
 Each file holds: `in.*` inputs, `sd.*` the reference module's state_dict,
 `out.*` reference outputs, `meta` (JSON: constructor arguments).
@@ -169,9 +169,74 @@ def sparse_edge_cases():
          {k: v.to(torch.int32) for k, v in outs.items()})
 
 
+def reference_cross_check(dense, sparse):
+    """What the oracle is pinned against (tests/test_oracle_pins.py): kNN matrices and DynConv2d outputs on random
+    shapes, every GENConv aggregator, the sparse kNN graph builder; and the constructor signatures and the
+    DenseDeepGCN state_dict layout the drop-in API is pinned against (tests/test_host_cpu.py)."""
+    g = torch.Generator().manual_seed(11)
+    ins, sd, outs = {}, {}, {}
+    for i, (B, C, N, k, d) in enumerate([(1, 5, 77, 3, 2), (3, 20, 130, 7, 1), (2, 3, 64, 8, 8)]):
+        x = torch.randn(B, C, N, 1, generator=g)
+        ins["x%d" % i] = x
+        outs["knn%d" % i] = dense.dense_knn_matrix(x, k * d)
+        for conv in ("edge", "mr"):
+            torch.manual_seed(3)
+            mod = dense.DynConv2d(C, 9, k, d, conv, "leakyrelu", "batch", True).eval()
+            with torch.no_grad():
+                outs["dyn%d_%s" % (i, conv)] = mod(x)
+            sd.update({"dyn%d_%s.%s" % (i, conv, key): v for key, v in mod.state_dict().items()})
+    x = torch.randn(90, 12, generator=g)
+    ei = torch.randint(0, 90, (2, 500), generator=g)
+    ins["xs"], ins["ei"] = x, ei
+    for aggr in ("softmax", "softmax_sg", "softmax_sum", "power", "power_sum", "add", "mean", "max"):
+        torch.manual_seed(4)
+        mod = sparse.GENConv(12, 12, aggr=aggr, t=0.3, learn_t=True, p=2.0, y=0.2, msg_norm=True).eval()
+        with torch.no_grad():
+            outs["gen_" + aggr] = mod(x, ei)
+        sd.update({"gen_%s.%s" % (aggr, key): v for key, v in mod.state_dict().items()})
+    te = sys.modules["gcn_lib.sparse.torch_edge"]
+    xs = torch.randn(3 * 50, 6, generator=g)
+    bs = torch.arange(3).repeat_interleave(50)
+    ins["xg"] = xs
+    for k, d in ((4, 1), (3, 4)):
+        outs["graph_%d_%d" % (k, d)] = te.DilatedKnnGraph(k, d)(xs, bs)
+    save("ref_random_shapes", {}, ins, sd, outs)
+
+    import inspect
+    import types
+    sigs = {}
+    for mod, names in ((dense, ("DenseDilated", "DenseDilatedKnnGraph", "DilatedKnnGraph", "MRConv2d", "EdgeConv2d",
+                                "GraphConv2d", "DynConv2d", "PlainDynBlock2d", "ResDynBlock2d", "DenseDynBlock2d",
+                                "BasicConv")),
+                       (sparse, ("GENConv", "MsgNorm", "MLP"))):
+        for n in names:
+            sigs[n] = [[p.name, p.default if p.default is not inspect.Parameter.empty else "<empty>"]
+                       for p in inspect.signature(getattr(mod, n).__init__).parameters.values()]
+    opt = dict(n_filters=16, k=4, act="relu", norm="batch", bias=True, epsilon=0.2, stochastic=True, conv="edge",
+               n_blocks=3, block="res", in_channels=9, n_classes=13, dropout=0.3)
+    src = open(os.path.join(ref_shims.REFERENCE_ROOT, "examples/sem_seg_dense/architecture.py")).read()
+    src = src.split('if __name__ == "__main__"')[0].replace("import __init__\n", "")
+    ns = {"__name__": "ref_arch"}
+    sys.path.insert(0, ref_shims.REFERENCE_ROOT)
+    try:
+        exec(compile(src, "ref_architecture.py", "exec"), ns)
+    finally:
+        sys.path.remove(ref_shims.REFERENCE_ROOT)
+    model = ns["DenseDeepGCN"](types.SimpleNamespace(**opt))
+    layout = [[key, list(v.shape)] for key, v in model.state_dict().items()]
+    with open(os.path.join(HERE, "ref_api.json"), "w") as fh:   # one class / one state_dict entry per line
+        fh.write('{"signatures": {\n')
+        fh.write(",\n".join("  %s: %s" % (json.dumps(k), json.dumps(v)) for k, v in sigs.items()))
+        fh.write('\n},\n"semseg_opt": %s,\n"semseg_state_dict": [\n' % json.dumps(opt))
+        fh.write(",\n".join("  %s" % json.dumps(e) for e in layout))
+        fh.write("\n]}\n")
+    print("wrote ref_api.json")
+
+
 if __name__ == "__main__":
     torch.set_num_threads(8)
     dense, sparse = ref_shims.load_reference()
     dense_cases(dense)
     sparse_cases(sparse)
     sparse_edge_cases()
+    reference_cross_check(dense, sparse)

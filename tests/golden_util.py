@@ -22,9 +22,19 @@ class Case:
             grp, name = key.split(".", 1)
             t = torch.from_numpy(z[key])
             {"in": self.ins, "sd": self.sd, "out": self.outs}[grp][name] = t
+        for name, (seed, shape) in self.meta.get("seeded", {}).items():
+            self.sd[name] = seeded_weight(seed, shape)
 
     def __repr__(self):
         return self.name
+
+
+def seeded_weight(seed, shape):
+    """A large weight of a golden model, not stored but drawn from its seed (keeps every golden file small):
+    normal with std 1/sqrt(fan_in)."""
+    g = torch.Generator().manual_seed(seed)
+    fan_in = max(1, int(np.prod(shape[1:])))
+    return torch.randn(*shape, generator=g) / float(np.sqrt(fan_in))
 
 
 def names(prefix):

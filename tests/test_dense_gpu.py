@@ -281,7 +281,7 @@ def test_large_k_at_full_cloud_size_vs_oracle(k, d, conv):
                                    (1, 16, 8192, 10, 1),      # N > 4096: unpacked (key, index) list entries
                                    (1, 8, 4224, 20, 2)])      # unpacked entries, K = 40 (list length 56)
 def test_tensor_core_prefilter_equals_exact_fp32_path(shape):
-    """The tcgen05 pre-filter is certified + re-ranked in exact fp32, so its neighbour lists
+    """The tensor-core pre-filter is certified + re-ranked in exact fp32, so its neighbour lists
     must be IDENTICAL (not just adjudicated-equal) to those of the pure fp32 FMA kernel."""
     from deep_gcns_torch_b200 import _native
     from deep_gcns_torch_b200.gcn_lib import dense as D
@@ -310,6 +310,33 @@ def test_tensor_core_prefilter_equals_exact_fp32_path(shape):
             torch.testing.assert_close(y, y_ref, rtol=1e-5, atol=1e-6)
     finally:
         _native.set_knn_path("auto")
+
+
+@pytest.mark.parametrize("path", ["tc", "tc1"])
+def test_tensor_core_prefilter_certifies_random_clouds(path):
+    """The exact completion kernel makes every answer right whatever the pre-filter certifies, so parity alone
+    cannot see a pre-filter that certifies nothing: on random clouds at most 1e-3 of the queries may be left to
+    it - set-only consumer (EdgeConv, eval), index output, and K = 40 (list of 56)."""
+    from deep_gcns_torch_b200 import _native
+    from deep_gcns_torch_b200.gcn_lib import dense as D
+    g = torch.Generator().manual_seed(77)
+    x = torch.randn(4, 64, 4096, 1, generator=g).cuda()
+    torch.manual_seed(0)
+    conv = D.DynConv2d(64, 64, 20, 1, "edge", "relu", "batch", True).cuda().eval()
+    _native.set_knn_path(path)
+    _native.tc_certification(True)
+    try:
+        _native.tc_certification_read()
+        with torch.no_grad():
+            conv(x)
+            D.DenseDilatedKnnGraph(20, 1)(x)
+            D.DenseDilatedKnnGraph(20, 2)(x)
+        failed, queries = _native.tc_certification_read()
+    finally:
+        _native.tc_certification(False)
+        _native.set_knn_path("auto")
+    assert queries == 3 * 4 * 4096, queries
+    assert failed <= 1e-3 * queries, (failed, queries)
 
 
 @pytest.mark.parametrize("cfg", [
@@ -431,8 +458,8 @@ def test_block_epilogues_fused_into_the_consumer(cfg):
 
 
 @pytest.mark.parametrize("cfg", [
-    # B, C, c_out, N, k, d, conv          (four-tile kernel: C % 8 == 0, K <= 20, c_out in {32, 64, 128})
-    (2, 64, 64, 4096, 20, 1, "edge"),     # the headline layer shape: 8 CTAs x 4 warpgroups per cloud
+    # B, C, c_out, N, k, d, conv          (multi-tile kernel: C % 8 == 0, K <= 20, c_out in {32, 64, 128})
+    (2, 64, 64, 4096, 20, 1, "edge"),     # the headline layer shape: 16 CTAs x 2 warpgroups per cloud
     (3, 64, 64, 1024, 10, 2, "edge"),     # dilation inside the kernel's rank selection (K = 20)
     (2, 32, 128, 640, 9, 1, "edge"),      # list of 16; 5 query tiles: the second CTA runs one warpgroup
     (1, 16, 32, 384, 16, 1, "edge"),      # 3 query tiles: one CTA with an idle warpgroup
@@ -441,7 +468,7 @@ def test_block_epilogues_fused_into_the_consumer(cfg):
     (1, 40, 64, 2048, 4, 1, "edge"),      # C = 40 -> three K=16 blocks of channels, zero padded
 ])
 def test_four_tile_kernel_equals_tile_per_cta_and_fp32_paths(cfg):
-    """knn_tc4_kernel (four query tiles per CTA, producer warp + four filter warpgroups, sorting-network flush)
+    """knn_tc4_kernel (two query tiles per CTA, TMA producer warp + two filter warpgroups, sorting-network flush)
     must return the neighbour lists of knn_tc_kernel and of the pure fp32 kernel bit for bit, and the features
     of knn_tc_kernel bit for bit (same consumer code on the same lists)."""
     from deep_gcns_torch_b200 import _native

@@ -94,43 +94,24 @@ def test_sparse_state_dict_compat(name):
     assert isinstance(getattr(mod, "t", 1.0), (float, torch.nn.Parameter))
 
 
-@pytest.mark.skipif(not ref_shims.reference_available(), reason="reference tree absent (GPU box)")
-def test_signatures_match_live_reference():
+def test_signatures_match_reference():
+    """Constructor signatures of the drop-in classes and the state_dict layout of a reference model stack
+    (examples/sem_seg_dense DenseDeepGCN) against the unmodified reference (golden ref_api.json)."""
     import inspect
+    import json
+    from bench_models import ResGCN28
     from deep_gcns_torch_b200.gcn_lib import dense as D, sparse as S
-    rd, rs = ref_shims.load_reference()
-    pairs = [(getattr(D, n), getattr(rd, n)) for n in
-             ("DenseDilated", "DenseDilatedKnnGraph", "DilatedKnnGraph", "MRConv2d", "EdgeConv2d", "GraphConv2d",
-              "DynConv2d", "PlainDynBlock2d", "ResDynBlock2d", "DenseDynBlock2d", "BasicConv")]
-    pairs += [(getattr(S, n), getattr(rs, n)) for n in ("GENConv", "MsgNorm", "MLP")]
-    for mine, ref in pairs:
-        a, b = inspect.signature(mine.__init__), inspect.signature(ref.__init__)
-        assert [(p.name, p.default) for p in a.parameters.values()] == \
-               [(p.name, p.default) for p in b.parameters.values()], mine.__name__
-    # model stacks of the reference build on top of the drop-in classes unchanged
-    import types
-    opt = types.SimpleNamespace(n_filters=16, k=4, act="relu", norm="batch", bias=True, epsilon=0.2,
-                                stochastic=True, conv="edge", n_blocks=3, block="res", in_channels=9,
-                                n_classes=13, dropout=0.3)
-    src = open(os.path.join(ref_shims.REFERENCE_ROOT, "examples/sem_seg_dense/architecture.py")).read()
-    src = src.split('if __name__ == "__main__"')[0].replace("import __init__\n", "")
-    src = src.replace("from gcn_lib.dense import", "from deep_gcns_torch_b200.gcn_lib.dense import")
-    ns = {}
-    exec(compile(src, "architecture.py", "exec"), ns)
-    mine = ns["DenseDeepGCN"](opt)
-    import sys
-    sys.path.insert(0, os.path.join(ref_shims.REFERENCE_ROOT, "examples/sem_seg_dense"))
-    ref_src = open(os.path.join(ref_shims.REFERENCE_ROOT, "examples/sem_seg_dense/architecture.py")).read()
-    ref_src = ref_src.split('if __name__ == "__main__"')[0].replace("import __init__\n", "")
-    ns2 = {"__name__": "ref_arch"}
-    sys.path.insert(0, ref_shims.REFERENCE_ROOT)
-    try:
-        exec(compile(ref_src, "ref_architecture.py", "exec"), ns2)
-    finally:
-        sys.path.remove(ref_shims.REFERENCE_ROOT)
-    theirs = ns2["DenseDeepGCN"](opt)
-    assert list(mine.state_dict().keys()) == list(theirs.state_dict().keys())
-    mine.load_state_dict(theirs.state_dict(), strict=True)
+    with open(os.path.join(gu.GOLDEN_DIR, "ref_api.json")) as fh:
+        ref = json.load(fh)
+    for name, params in ref["signatures"].items():
+        mine = getattr(S if name in ("GENConv", "MsgNorm", "MLP") else D, name)
+        a = inspect.signature(mine.__init__)
+        assert [[p.name, p.default if p.default is not inspect.Parameter.empty else "<empty>"]
+                for p in a.parameters.values()] == params, name
+    # the reference's model stack, assembled from the drop-in classes, has the reference's state_dict layout
+    opt = ref["semseg_opt"]
+    mine = ResGCN28(D, opt["in_channels"], opt["n_classes"], opt["k"], opt["n_filters"], opt["n_blocks"])
+    assert [[k, list(v.shape)] for k, v in mine.state_dict().items()] == ref["semseg_state_dict"]
 
 
 def test_bench_line_carries_every_contract_key():
@@ -152,7 +133,7 @@ def test_bench_line_carries_every_contract_key():
         steps, warmup = 20, 1
 
     loc = dict(world=2, args=Args, ms=11.4, ms_e2e=12.7, clk={"sm_mhz": 1965.0}, achieved=220.0, peak=6563.9,
-               traffic=72000000, peak_src="measured", kernel_ms=0.507, tensor_peak=1691.8, sm_max=1965.0,
+               traffic=72000000, peak_src="measured", tensor_src="measured", kernel_ms=0.507, tensor_peak=1691.8, sm_max=1965.0,
                hbm_achieved=66.0, tensor_flop=1.1e11, numa={"numa_node": 0})
     out = eval(compile(ast.Expression(lit), path, "eval"), g, loc)
     json.dumps(out)

@@ -245,7 +245,7 @@ def test_partitioned_layer_emulated_on_one_gpu():
 
 @pytest.mark.parametrize("N,K,M", [(1000, 128, 128), (129, 64, 32), (5000, 256, 64), (3000, 64, 256), (128 * 150 + 7, 128, 64), (1, 64, 96)])
 def test_tcgen05_row_linear_with_bias_and_skip(N, K, M):
-    """dgcn_linear_residual (tcgen05, two-plane bf16 split of both operands) against an fp64 Linear: the split
+    """dgcn_linear_residual (wgmma, two-plane bf16 split of both operands) against an fp64 Linear: the split
     leaves <= ~2^-16 * sum|a||w| of error, far inside the 1e-3 parity tolerance; bias / skip optional; rows beyond
     the last full 128-row tile; out aliasing res."""
     from deep_gcns_torch_b200 import _native
@@ -265,6 +265,9 @@ def test_tcgen05_row_linear_with_bias_and_skip(N, K, M):
         err = (out.double() - ref).abs()
         assert bool((err <= 4e-5 * mag + 1e-6 * ref.abs() + 1e-6).all()), float((err / (mag + 1e-9)).max())
         torch.testing.assert_close(out, ref.float(), rtol=1e-3, atol=1e-4)
+    b_odd = torch.cat((torch.zeros(1, device="cuda"), b))[1:]            # bias at an odd float offset (4-byte aligned)
+    torch.testing.assert_close(_native.linear_residual(a, w, b_odd, h),
+                               (a.double() @ w.double().t() + b.double() + h.double()).float(), rtol=1e-3, atol=1e-4)
     buf = h.clone()
     _native.linear_residual(a, w, b, buf, out=buf)                     # in place on the skip tensor
     torch.testing.assert_close(buf, (a.double() @ w.double().t() + b.double() + h.double()).float(), rtol=1e-3, atol=1e-4)

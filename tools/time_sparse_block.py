@@ -49,15 +49,15 @@ def main():
         res["addmm_beta_ms"] = timeit(lambda: torch.addmm(h, a, lin.weight.t(), out=out))
         res["addmm_beta_bias_ms"] = timeit(lambda: torch.addmm(h, a, lin.weight.t(), out=out).add_(lin.bias))
         res["linear_out_add_ms"] = timeit(lambda: F.linear(a, lin.weight, lin.bias).add_(h))
-        res["tcgen05_linear_residual_ms"] = timeit(lambda: _native.linear_residual(a, lin.weight, lin.bias, h, out=out))
+        res["tc_linear_residual_ms"] = timeit(lambda: _native.linear_residual(a, lin.weight, lin.bias, h, out=out))
         _native.kernel_timing(True)
         _native.kernel_timing_read("linear")
         for _ in range(10):
             _native.linear_residual(a, lin.weight, lin.bias, h, out=out)
         ms, n = _native.kernel_timing_read("linear")
         _native.kernel_timing(False)
-        res["tcgen05_linear_kernel_ms"] = ms / max(n, 1)
-        res["tcgen05_linear_hbm_gbs"] = 3 * N * C * 4 / (ms / max(n, 1) * 1e-3) / 1e9
+        res["tc_linear_kernel_ms"] = ms / max(n, 1)
+        res["tc_linear_hbm_gbs"] = 3 * N * C * 4 / (ms / max(n, 1) * 1e-3) / 1e9
     print(json.dumps(res))
 
 

@@ -43,7 +43,7 @@ size_t knn_workspace_bytes(int64_t B, int64_t C, int64_t N, int64_t K) {
     const int64_t cpad = (C + 15) / 16 * 16;
     bytes += align_up(static_cast<size_t>(B) * TC_PLANES * cpad * N * 2, 256);   // bf16 planes
     bytes += align_up(static_cast<size_t>(B) * N * C * 4, 256);          // node-major copy
-    bytes += align_up(static_cast<size_t>(B) * 4, 256);                  // per-cloud max |x|^2
+    bytes += align_up(static_cast<size_t>(B) * 8, 256);                  // per-cloud max |x|^2, max fp16 rounding error
     bytes += align_up(static_cast<size_t>(B) * 8 * N * 2, 256);          // -|x|^2/2 operand block
     bytes += align_up(static_cast<size_t>(B) * N * 4 + 256, 256);        // fail counter + list
   }
@@ -98,17 +98,18 @@ static EncodeTiledFn tensor_map_encoder() {
   }
   return reinterpret_cast<EncodeTiledFn>(fn);
 }
-// bf16 matrix (rows, cols) row-major -> tensor map with boxes of 64 columns (128 bytes) x box_rows rows, SWIZZLE_128B:
-// a box lands in shared memory as box_rows x 128 B rows with the 16-byte chunks XOR-swizzled by (row & 7), which is
-// the canonical MN-major wgmma layout of one 64-wide MN block.
-static int make_plane_map(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int box_rows) {
+// 16-bit matrix (rows, cols) row-major, elements of type `dtype` (bf16 or fp16) -> tensor map with boxes of 64 columns
+// (128 bytes) x box_rows rows, SWIZZLE_128B: a box lands in shared memory as box_rows x 128 B rows with the 16-byte
+// chunks XOR-swizzled by (row & 7), which is the canonical MN-major wgmma layout of one 64-wide MN block.
+static int make_plane_map(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int box_rows,
+                          CUtensorMapDataType dtype) {
   EncodeTiledFn enc = tensor_map_encoder();
   if (!enc) return DGCN_ERR_UNSUPPORTED;
   const cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
   const cuuint64_t strides[1] = {static_cast<cuuint64_t>(cols) * 2};
   const cuuint32_t box[2] = {64u, static_cast<cuuint32_t>(box_rows)};
   const cuuint32_t estr[2] = {1u, 1u};
-  const CUresult rc = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
+  const CUresult rc = enc(map, dtype, 2, const_cast<void*>(base), dims, strides, box, estr,
                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return rc == CUDA_SUCCESS ? DGCN_OK : DGCN_ERR_CUDA;
@@ -121,36 +122,50 @@ static int launch_knn_tc(KnnArgs& a, Workspace& ws, cudaStream_t stream, const f
   const int cpad = (C + 15) / 16 * 16;
   __nv_bfloat16* planes = ws.take<__nv_bfloat16>(static_cast<size_t>(B) * TC_PLANES * cpad * N);
   float* xt_own = xt ? nullptr : ws.take<float>(static_cast<size_t>(B) * N * C);
-  float* sqmax = ws.take<float>(static_cast<size_t>(B));
+  float* sqmax = ws.take<float>(static_cast<size_t>(B) * 2);   // max |x|^2, max fp16 rounding error |e|^2
   __nv_bfloat16* sqp = ws.take<__nv_bfloat16>(static_cast<size_t>(B) * 8 * N);
   int* fail = ws.take<int>(static_cast<size_t>(B) * N + 64);
   if (!ws.ok) return DGCN_ERR_WORKSPACE;
   DGCN_CUDA_TRY(cudaMemsetAsync(fail, 0, 256, stream));
-  DGCN_CUDA_TRY(cudaMemsetAsync(sqmax, 0, static_cast<size_t>(B) * 4, stream));
-  // sq, bf16 planes, node-major copy and max |x|^2 in one pass over x (sq overwrites what the caller computed)
+  DGCN_CUDA_TRY(cudaMemsetAsync(sqmax, 0, static_cast<size_t>(B) * 8, stream));
+  if (!xt) xt = xt_own;
+  // The kernel is chosen before the prologue: knn_tc4_kernel reads one fp16 plane, knn_tc_kernel the two bf16 planes.
+  // list length = K + certification margin
+  // (a margin of 4 ranks leaves ~1e-5 of the queries of a random 64-d cloud uncertified, 8 ranks none)
+  const int kp = K <= 9 ? 16 : K <= 20 ? 28 : K <= 32 ? 40 : 56;
+  const int kp4 = knn_tc4_list_len(K);
+  const bool packed = N <= 4096;
+  const bool wide = epilogue_wide_ok(a);
+  const bool xt32 = (reinterpret_cast<uintptr_t>(xt) & 31) == 0;
+  // T4_GROUPS query tiles per CTA, warp specialised (knn_tc4.cuh), where its smaller work area and fixed consumer fit
+  const bool train = a.epi.mode == EPI_EDGE && a.epi.norm == DGCN_NORM_BATCH_TRAIN;
+  const bool quad = !a.tc_tile_per_cta && packed && wide && !train && xt32 && (C & 7) == 0 && knn_tc4_list_ok(kp4, a.k);
+  // sq, operand plane(s), node-major copy and max |x|^2 in one pass over x (sq overwrites what the caller computed)
   if (pqf) {   // the EdgeConv node GEMM rides on the same pass over x
     const size_t smem = (static_cast<size_t>(TC_MAX_C) * 68 + static_cast<size_t>(C) * pqf->M) * 4;
     DGCN_ENSURE_SMEM((tc_prologue_pq_kernel), smem);
     tc_prologue_pq_kernel<<<dim3(N / 64, B), 256, smem, stream>>>(a.x, a.sb, a.sc, C, cpad, N, const_cast<float*>(a.sq),
-                                                                  planes, xt ? nullptr : xt_own, sqmax, sqp, *pqf);
+                                                                  planes, xt_own, sqmax, sqp, *pqf, quad);
   } else {
     tc_prologue_kernel<<<dim3(ceil_div(N, 32), B), 256, 0, stream>>>(a.x, a.sb, a.sc, C, cpad, N,
                                                                  const_cast<float*>(a.sq), planes,
-                                                                 xt ? nullptr : xt_own, sqmax, sqp);
+                                                                 xt_own, sqmax, sqp, quad);
   }
   DGCN_LAUNCH_CHECK();
-  if (!xt) xt = xt_own;
   TcArgs t{};
   {
-    int rc = make_plane_map(&t.tm_planes, planes, static_cast<int64_t>(B) * TC_PLANES * cpad, N, cpad);
-    if (rc == DGCN_OK) rc = make_plane_map(&t.tm_sqp, sqp, static_cast<int64_t>(B) * 8, N, 8);
+    int rc = quad ? make_plane_map(&t.tm_planes, planes, static_cast<int64_t>(B) * cpad, N, cpad,
+                                   CU_TENSOR_MAP_DATA_TYPE_FLOAT16)
+                  : make_plane_map(&t.tm_planes, planes, static_cast<int64_t>(B) * TC_PLANES * cpad, N, cpad,
+                                   CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
+    if (rc == DGCN_OK) rc = make_plane_map(&t.tm_sqp, sqp, static_cast<int64_t>(B) * 8, N, 8, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
     if (rc != DGCN_OK) return rc;
   }
   t.a = a;
   t.planes = planes;
   t.sqp = sqp;
   t.xt = xt;
-  t.xt32 = (reinterpret_cast<uintptr_t>(xt) & 31) == 0 ? 1 : 0;
+  t.xt32 = xt32 ? 1 : 0;
   t.sqmax = sqmax;
   t.Cpad = cpad;
   t.fail_count = fail;
@@ -160,21 +175,14 @@ static int launch_knn_tc(KnnArgs& a, Workspace& ws, cudaStream_t stream, const f
   {
     KernelTimer timer(stream, "knn");
     const int nch = a.epi.mode == EPI_MR ? a.epi.c_in : a.epi.c_out;
-    t.wide = epilogue_wide_ok(a) ? 1 : 0;
+    t.wide = wide ? 1 : 0;
     t.flush_early = TC_FLUSH_EARLY;
     t.flush_late = TC_FLUSH_LATE;
-    // list length = K + certification margin
-    // (a margin of 4 ranks leaves ~1e-5 of the queries of a random 64-d cloud uncertified, 8 ranks none)
-    const int kp = K <= 9 ? 16 : K <= 20 ? 28 : K <= 32 ? 40 : 56;
     t.work_bytes = static_cast<int>(tc_work_bytes(kp, a.k, t.wide != 0, nch));
     const size_t smem = static_cast<size_t>(t.work_bytes) + sizeof(TcTail) + 1024;
-    const bool packed = N <= 4096;
-    // T4_GROUPS query tiles per CTA, warp specialised (knn_tc4.cuh), where its smaller work area and fixed consumer fit
-    const bool train = a.epi.mode == EPI_EDGE && a.epi.norm == DGCN_NORM_BATCH_TRAIN;
-    const bool quad = !a.tc_tile_per_cta && packed && t.wide && !train && t.xt32 && (C & 7) == 0 && knn_tc4_list_ok(kp, a.k);
     int rc;
     if (quad) {
-      rc = launch_knn_tc4(kp, t, dim3(static_cast<unsigned>(ceil_div(N / TILE, T4_GROUPS)), B), stream);
+      rc = launch_knn_tc4(kp4, t, dim3(static_cast<unsigned>(ceil_div(N / TILE, T4_GROUPS)), B), stream);
     } else
     switch (kp) {
       case 16: rc = launch_knn_tc_kp16(packed, t, grid, smem, stream); break;

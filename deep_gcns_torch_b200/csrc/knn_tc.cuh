@@ -4,7 +4,8 @@
 //
 //   tc_prologue(_pq)  one pass over x: x = hi + mid (two bf16 planes, channel-major like x, channels
 //                     zero-padded to a multiple of 16; the three products hi*hi, hi*mid, mid*hi
-//                     reproduce x_i.x_j to ~2^-16 relative), |x|^2, the operand block that folds
+//                     reproduce x_i.x_j to ~2^-16 relative) - or, for knn_tc4_kernel (knn_tc4.cuh), one
+//                     fp16 plane of the same layout - |x|^2, the operand block that folds
 //                     -|x_j|^2/2 into the product, the node-major fp32 copy, max |x|^2 (and the
 //                     EdgeConv node GEMM).
 //   knn_tc_kernel     one 128-thread CTA (one warpgroup) = 128 queries of a cloud.  Query planes stay
@@ -29,6 +30,7 @@
 #pragma once
 #include <cuda.h>          // CUtensorMap (type only: the encoder comes from cudaGetDriverEntryPoint)
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include "knn.cuh"
 #include "wgmma.cuh"
 
@@ -137,27 +139,47 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 // channels >= C are zero.  Three bf16 products hi*hi, hi*mid, mid*hi reproduce x_i.x_j to
 // 2^-15 relative to |x_i||x_j| in the worst case (two split residuals 2^-16 + the dropped mid*mid
 // term 2^-16) - a pre-filter accuracy, the ranking itself is redone in exact fp32.
+// knn_tc4_kernel instead reads ONE fp16 plane (B, 1, Cpad, N) (f16 = true below): its packed list entries keep
+// fewer bits than even a single fp16 product delivers (knn_tc4.cuh).
 constexpr int TC_PLANES = 2;
 
+// x -> fp16 operand, clamped to the finite range so that no inf or NaN ever reaches the MMA (a cloud with
+// max |x|^2 >= 2^30, where clamping may have happened, is never certified by knn_tc4_kernel)
+__device__ __forceinline__ __half tc_to_f16(float v) { return __float2half_rn(fminf(fmaxf(v, -65504.f), 65504.f)); }
+// Squared rounding error of one fp16 operand channel, an upper bound whether or not the MMA flushes subnormal
+// inputs to zero: |h - x|, or |x| where h is subnormal (flushed, the MMA reads 0 for x).
+__device__ __forceinline__ float tc_f16_err2(float v) {
+  const float h = __half2float(tc_to_f16(v));
+  float e = fabsf(h - v);
+  if (h != 0.f && fabsf(h) < 6.103515625e-05f) e = fmaxf(e, fabsf(v));
+  return e * e;
+}
+
 // One pass over x for everything the tensor-core path needs: sq (B,N) (same FMA chain as sqnorm_kernel),
-// the bf16 planes, the extra operand block sqp that folds -|x_j|^2/2 into the tensor-core product, the
-// node-major copy xt (optional) and the per-cloud max of sq (atomicMax on the bits of a non-negative
-// float; sqmax must be zero-initialised).  Block = 32 points x all channels (C <= 64).
+// the bf16 planes (f16: the fp16 plane instead, written into the same buffer), the extra operand block sqp that
+// folds -|x_j|^2/2 into the tensor-core product, the node-major copy xt (optional) and the per-cloud max of sq
+// (atomicMax on the bits of a non-negative float; sqmax (2B) must be zero-initialised); with f16 also, in
+// sqmax[B + b], the per-cloud max of |e|^2, e = the fp16 plane's rounding error (tc_f16_err2).  Block = 32 points x
+// all channels (C <= 64).
 #ifndef DGCN_TEMPLATES_ONLY
 __global__ void __launch_bounds__(256) tc_prologue_kernel(const float* __restrict__ x, int64_t sb, int64_t sc, int C,
                                                          int Cpad, int N, float* __restrict__ sq,
                                                          __nv_bfloat16* __restrict__ planes, float* __restrict__ xt,
-                                                         float* __restrict__ sqmax, __nv_bfloat16* __restrict__ sqp) {
+                                                         float* __restrict__ sqmax, __nv_bfloat16* __restrict__ sqp,
+                                                         bool f16) {
   __shared__ float tile[TC_MAX_C][33];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const int b = blockIdx.y, n0 = blockIdx.x * 32, n = n0 + tx;
   const int64_t plane = static_cast<int64_t>(Cpad) * N;
   __nv_bfloat16* pb = planes + static_cast<int64_t>(b) * TC_PLANES * plane;
+  __half* ph = reinterpret_cast<__half*>(planes) + static_cast<int64_t>(b) * plane;
   for (int c = ty; c < Cpad; c += 8) {
     float v = 0.f;
     if (c < C && n < N) v = __ldg(x + b * sb + c * sc + n);
     if (c < C) tile[c][tx] = v;
-    if (n < N) {
+    if (n < N && f16) {
+      ph[static_cast<int64_t>(c) * N + n] = tc_to_f16(v);
+    } else if (n < N) {
       const __nv_bfloat16 hi = __float2bfloat16_rn(v);
       pb[static_cast<int64_t>(c) * N + n] = hi;
       pb[plane + static_cast<int64_t>(c) * N + n] = __float2bfloat16_rn(v - __bfloat162float(hi));
@@ -165,8 +187,13 @@ __global__ void __launch_bounds__(256) tc_prologue_kernel(const float* __restric
   }
   __syncthreads();
   if (ty == 0) {
-    float s = 0.f;
+    float s = 0.f, e2 = 0.f;
     for (int c = 0; c < C; ++c) s = fmaf(tile[c][tx], tile[c][tx], s);
+    if (f16) {
+      for (int c = 0; c < C; ++c) e2 += tc_f16_err2(tile[c][tx]);
+      const float em = warp_max(n < N ? e2 : 0.f);
+      if (tx == 0) atomicMax(reinterpret_cast<unsigned int*>(sqmax + gridDim.y + b), __float_as_uint(em));
+    }
     if (n < N) {
       sq[static_cast<int64_t>(b) * N + n] = s;
       // rows 0..2 of the (B, 8, N) extra operand block: -|x|^2 / 2 as three bf16 terms (2^-24 relative)
@@ -209,7 +236,7 @@ __global__ void __launch_bounds__(256, 4) tc_prologue_pq_kernel(const float* __r
                                                             int Cpad, int N, float* __restrict__ sq,
                                                             __nv_bfloat16* __restrict__ planes, float* __restrict__ xt,
                                                             float* __restrict__ sqmax, __nv_bfloat16* __restrict__ sqp,
-                                                            const ProloguePq g) {
+                                                            const ProloguePq g, bool f16) {
   extern __shared__ __align__(16) float pq_smem[];
   constexpr int XLD = 68;
   float* xs = pq_smem;                       // [C][XLD]
@@ -219,12 +246,17 @@ __global__ void __launch_bounds__(256, 4) tc_prologue_pq_kernel(const float* __r
   const int M = g.M;
   const int64_t plane = static_cast<int64_t>(Cpad) * N;
   __nv_bfloat16* pb = planes + static_cast<int64_t>(b) * TC_PLANES * plane;
+  __half* ph = reinterpret_cast<__half*>(planes) + static_cast<int64_t>(b) * plane;
   if (((reinterpret_cast<uintptr_t>(x) & 7) | (sb & 1) | (sc & 1)) == 0) {
     // two adjacent points per thread: 8-byte loads, one bf16x2 store per plane (each half rounded like the scalar path)
     const int lane = tid & 31, wrp = tid >> 5, n = n0 + 2 * lane;
     for (int c = wrp; c < Cpad; c += 8) {
       const float2 v = c < C ? __ldg(reinterpret_cast<const float2*>(x + b * sb + c * sc + n)) : make_float2(0.f, 0.f);
       if (c < C) *reinterpret_cast<float2*>(xs + c * XLD + 2 * lane) = v;
+      if (f16) {
+        *reinterpret_cast<__half2*>(ph + static_cast<int64_t>(c) * N + n) = __halves2half2(tc_to_f16(v.x), tc_to_f16(v.y));
+        continue;
+      }
       const __nv_bfloat162 hi = __floats2bfloat162_rn(v.x, v.y);
       const __nv_bfloat162 mid = __floats2bfloat162_rn(v.x - __low2float(hi), v.y - __high2float(hi));
       *reinterpret_cast<__nv_bfloat162*>(pb + static_cast<int64_t>(c) * N + n) = hi;
@@ -235,6 +267,10 @@ __global__ void __launch_bounds__(256, 4) tc_prologue_pq_kernel(const float* __r
     for (int c = ty; c < Cpad; c += 4) {
       const float v = c < C ? __ldg(x + b * sb + c * sc + n) : 0.f;
       if (c < C) xs[c * XLD + tx] = v;
+      if (f16) {
+        ph[static_cast<int64_t>(c) * N + n] = tc_to_f16(v);
+        continue;
+      }
       const __nv_bfloat16 hi = __float2bfloat16_rn(v);
       pb[static_cast<int64_t>(c) * N + n] = hi;
       pb[plane + static_cast<int64_t>(c) * N + n] = __float2bfloat16_rn(v - __bfloat162float(hi));
@@ -248,6 +284,12 @@ __global__ void __launch_bounds__(256, 4) tc_prologue_pq_kernel(const float* __r
     float s = 0.f;
     for (int c = 0; c < C; ++c) s = fmaf(xs[c * XLD + tid], xs[c * XLD + tid], s);
     sq[static_cast<int64_t>(b) * N + n] = s;
+    if (f16) {
+      float e2 = 0.f;
+      for (int c = 0; c < C; ++c) e2 += tc_f16_err2(xs[c * XLD + tid]);
+      const float em = warp_max(e2);
+      if ((tid & 31) == 0) atomicMax(reinterpret_cast<unsigned int*>(sqmax + gridDim.y + b), __float_as_uint(em));
+    }
     __nv_bfloat16* sp = sqp + static_cast<int64_t>(b) * 8 * N + n;
     float rem = -0.5f * s;
 #pragma unroll
@@ -326,13 +368,14 @@ __device__ __forceinline__ void ldg_f8(const float* p, float (&w)[8]) {
 }
 
 struct TcArgs {
-  CUtensorMap tm_planes;         // bf16 (B*2*Cpad rows, N) row-major, box 64 points x Cpad rows, SWIZZLE_128B
+  CUtensorMap tm_planes;         // bf16 (B*2*Cpad rows, N) - fp16 (B*Cpad rows, N) for knn_tc4_kernel - row-major,
+                                 // box 64 points x Cpad rows, SWIZZLE_128B
   CUtensorMap tm_sqp;            // bf16 (B*8 rows, N), box 64 points x 8 rows, SWIZZLE_128B
   KnnArgs a;
-  const __nv_bfloat16* planes;   // (B,2,Cpad,N)
+  const __nv_bfloat16* planes;   // (B,2,Cpad,N) bf16, or (B,1,Cpad,N) fp16 for knn_tc4_kernel
   const __nv_bfloat16* sqp;      // (B,8,N): rows 0..2 = bf16 split of -|x|^2/2, rest zero
   const float* xt;               // (B,N,C) node-major fp32 copy (exact re-rank)
-  const float* sqmax;            // (B)
+  const float* sqmax;            // (B) max |x|^2; knn_tc4_kernel: (2B), then the max fp16 rounding error |e|^2
   int Cpad;
   int wide;                      // consumer variant (cta_epilogue_wide)
   int work_bytes;                // size of the work area, see tc_work_bytes

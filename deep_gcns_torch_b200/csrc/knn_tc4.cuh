@@ -5,12 +5,19 @@
 //   sorting-network flush.  Two groups: the query planes, the per-group accumulator stage and candidate buffer of a
 //   third would not fit the 227 KB of shared memory an H100 block may use.
 //
+//   Operands: ONE fp16 plane (tc_prologue with f16), not knn_tc_kernel's bf16 (hi, mid) split.  The list entries keep
+//   20 bits of the distance, a resolution delta(v) = 2^-10 (v + |x_i|^2) (~0.14 at rank 20 of a 64-d normal cloud);
+//   the three-product bf16 split (~2^-14 relative, eps ~0.012 there) decided membership ~10x finer than the list can
+//   hold it; a single fp16 product (11-bit significand; with the per-query bound below, eps ~0.08) is of the same
+//   order as delta.  That is 10 instead of 26 m64n64k16 wgmma per half-tile and group at Cpad = 64, and half the
+//   operand bytes (TMA, shared memory, the wgmma's reads); the price is a list of 32 instead of 28 entries and a band of up to 16 instead of 12 (DESIGN.md 6).
+//
 //   producer warp            moves the operands by TMA: the query planes of the groups once, then 64-candidate
 //                            half-tiles into a two-stage ring (the stage of half-tile h+1 is refilled as soon as every
 //                            group has finished its wgmma on half-tile h-1, stage_free).
 //   filter warpgroup g       per half-tile: wait full[s], two m64n64k16 wgmma chains (query rows 0..63 and 64..127,
-//                            3*Cpad/16 + 1 each) against the stage, release the stage, the accumulators to the group's
-//                            shared-memory stage (row = query); thread r = query r of tile g reads 8 columns at a
+//                            Cpad/16 fp16 + 1 bf16 each) against the stage, release the stage, the accumulators to the
+//                            group's shared-memory stage (row = query); thread r = query r of tile g reads 8 columns at a
 //                            time, threshold test -> private candidate buffer (shared memory, slot-major).
 //                            FLUSH = sorting network instead of one insertion per entry: the batch (<= 16 entries
 //                            per lane, a second pass for slots 16..23) is bitonic-sorted in registers, min-merged
@@ -18,7 +25,7 @@
 //                            one 32-input bitonic merge - a fixed ~450 instructions per warp-wide flush whatever
 //                            the lanes' counts (the insertion loop costs ~80 per ROUND, rounds = the fullest
 //                            lane's count).
-//                            Then, per warpgroup (named barriers) in the group's own (now idle) query-plane memory:
+//                            Then, per warpgroup (named barriers) in the group's own (now idle) accumulator stage:
 //                            - set-only consumers (every rank kept, no index output, no self exclusion): membership
 //                              by interval arithmetic on the approximate list, exact fp32 chains only inside the
 //                              ambiguous band around rank K (DESIGN.md 6);
@@ -26,7 +33,7 @@
 //                              knn_tc_kernel;
 //                            and the fused consumer (cta_epilogue_wide).
 //
-// Eligibility (host side, launch_knn_tc): packed entries (N <= 4096), K <= 20 (list of 28 or 16), C % 8 == 0,
+// Eligibility (host side, launch_knn_tc): packed entries (N <= 4096), K <= 20 (list of 32 or 20), C % 8 == 0,
 // 32-byte aligned node-major copy, wide consumer, no train-mode statistics.  Everything else keeps knn_tc_kernel.
 #pragma once
 #include "knn_tc.cuh"
@@ -40,8 +47,9 @@ constexpr int T4_STAGES = 2;
 constexpr int T4_CAP = 24;                                       // candidate-buffer slots per thread
 constexpr int T4_FLUSH_AT = 16;                                  // flush when a lane holds this many (checked every 8 candidates)
 constexpr int T4_LIST = 32;                                      // register list length (power of two >= KP)
-constexpr int T4_QBYTES = TC_PLANES * 2 * TC_MAX_C * 128;        // 32 KB: query planes of one group
-constexpr int T4_STAGE_BYTES = TC_PLANES * TC_MAX_C * 128;       // 16 KB: one 64-candidate half-tile
+constexpr int T4_QBYTES = 2 * TC_MAX_C * 128;                    // 16 KB: fp16 query plane of one group (2 MN blocks)
+constexpr int T4_STAGE_BYTES = TC_MAX_C * 128;                   // 8 KB: one 64-candidate fp16 half-tile
+constexpr int T4_MB = 16;                                        // band entries a query may hold (set-only path)
 constexpr int T4_SX_BYTES = 16 * 128;                            // 2 KB: candidate-side extra K=16 block
 constexpr int T4_CBUF_BYTES = T4_CAP * 128 * 4;                  // 12 KB per group
 constexpr int T4_ACC_LD = 68;                                    // accumulator stage row: 64 columns + 4
@@ -60,6 +68,8 @@ constexpr size_t T4_SMEM_BYTES = static_cast<size_t>(T4_GROUPS) * T4_QBYTES + T4
                                  TC_XBLOCK_BYTES + static_cast<size_t>(T4_GROUPS) * (T4_CBUF_BYTES + T4_ACC_BYTES) +
                                  sizeof(T4Tail) + 1024;
 static_assert(T4_SMEM_BYTES <= 227 * 1024, "one CTA per SM");
+// after the loop a group's accumulator stage holds the band (exact keys + indices) or the exact-sorted list
+static_assert(T4_MB * TILE * (8 + 4) <= T4_ACC_BYTES && T4_LIST * TILE * 8 <= T4_ACC_BYTES, "work areas");
 
 // compare-exchange of two register entries (ascending)
 __device__ __forceinline__ void t4_ce(uint32_t& x, uint32_t& y) {
@@ -118,8 +128,8 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
   static_assert(KP <= T4_LIST && (KP & 1) == 0, "list length");
   extern __shared__ __align__(16) unsigned char smem_raw[];
   unsigned char* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // SWIZZLE_128B atoms: 1024-aligned
-  unsigned char* qbase = base;                                              // [group][plane][mn block][Cpad rows][128 B]
-  unsigned char* stage0 = qbase + T4_GROUPS * T4_QBYTES;                    // [stage][plane][Cpad rows][128 B]
+  unsigned char* qbase = base;                                              // [group][mn block][Cpad rows][128 B]
+  unsigned char* stage0 = qbase + T4_GROUPS * T4_QBYTES;                    // [stage][Cpad rows][128 B]
   unsigned char* sx0 = stage0 + T4_STAGES * T4_STAGE_BYTES;                 // [stage][16 rows][128 B]
   unsigned char* qx = sx0 + T4_STAGES * T4_SX_BYTES;                        // ones block, shared by the groups
   unsigned char* cbuf0 = qx + TC_XBLOCK_BYTES;                              // [group][slot][128 threads] u32
@@ -132,7 +142,7 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
   const int qt0 = blockIdx.x * T4_GROUPS;                                   // first query tile of this CTA
   const int ngroups = min(T4_GROUPS, N / TILE - qt0);
   const int H = N / T4_CT;
-  const int plane_q = 2 * Cpad * 128, plane_c = Cpad * 128;
+  const int plane_q = 2 * Cpad * 128, plane_c = Cpad * 128;               // fp16 query plane / candidate half-tile
 
   if (tid == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&t.tm_planes)) : "memory");
@@ -158,25 +168,20 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
 
   if (warp >= T4_GROUPS * 4) {
     // ================================ producer: TMA ================================
-    const uint32_t tile_bytes = static_cast<uint32_t>(2 * plane_c + 8 * 128);
+    const uint32_t tile_bytes = static_cast<uint32_t>(plane_c + 8 * 128);
     auto tma_tile = [&](int h) {
       const int s = h & 1;
       mbar_expect_tx(&sm.full[s], tile_bytes);
-#pragma unroll
-      for (int pl = 0; pl < TC_PLANES; ++pl)
-        tma_load_2d(smem_u32(stage0 + s * T4_STAGE_BYTES) + pl * plane_c, &t.tm_planes, h * T4_CT,
-                    (b * TC_PLANES + pl) * Cpad, &sm.full[s]);
+      tma_load_2d(smem_u32(stage0 + s * T4_STAGE_BYTES), &t.tm_planes, h * T4_CT, b * Cpad, &sm.full[s]);
       tma_load_2d(smem_u32(sx0 + s * T4_SX_BYTES), &t.tm_sqp, h * T4_CT, b * 8, &sm.full[s]);
     };
     if (t4_elect_one()) {
-      mbar_expect_tx(&sm.q_full, static_cast<uint32_t>(ngroups * 2 * plane_q));
+      mbar_expect_tx(&sm.q_full, static_cast<uint32_t>(ngroups * plane_q));
       for (int g = 0; g < ngroups; ++g)
 #pragma unroll
-        for (int pl = 0; pl < TC_PLANES; ++pl)
-#pragma unroll
-          for (int blk = 0; blk < 2; ++blk)
-            tma_load_2d(smem_u32(qbase + g * T4_QBYTES) + pl * plane_q + blk * (Cpad * 128), &t.tm_planes,
-                        (qt0 + g) * TILE + blk * 64, (b * TC_PLANES + pl) * Cpad, &sm.q_full);
+        for (int blk = 0; blk < 2; ++blk)
+          tma_load_2d(smem_u32(qbase + g * T4_QBYTES) + blk * (Cpad * 128), &t.tm_planes, (qt0 + g) * TILE + blk * 64,
+                      b * Cpad, &sm.q_full);
       tma_tile(0);
 #pragma unroll 1
       for (int h = 0; h + 1 < H; ++h) {                    // refill the other stage: its wgmma (half-tile h-1) must be done
@@ -285,26 +290,22 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
       const int s = h & 1;
       mbar_wait_hint(&sm.full[s], static_cast<uint32_t>((h >> 1) & 1), 1000u);
       {
-        // query rows 0..63 and 64..127 against the 64 staged candidates: hi*hi, hi*mid, mid*hi (mid*mid <= 2^-16
-        // |x_i||x_j| is inside eps), then + 1 x (-|x_j|^2/2)
+        // query rows 0..63 and 64..127 against the 64 staged candidates: one fp16 product x_i.x_j, then (bf16,
+        // into the same fp32 accumulators) + 1 x (-|x_j|^2/2)
         const uint32_t bbase = smem_u32(stage0 + s * T4_STAGE_BYTES);
         float d0[32], d1[32];
         wg_fence();
 #pragma unroll 1
         for (int kk = 0; kk < Cpad / 16; ++kk) {
-          const uint32_t ah = abase + kk * 2048, am = ah + plane_q, bh = bbase + kk * 2048, bm = bh + plane_c;
-          const uint64_t dbh = wg_desc_sw128(bh, Cpad * 128, 1024), dbm = wg_desc_sw128(bm, Cpad * 128, 1024);
+          const uint32_t ah = abase + kk * 2048;
+          const uint64_t db = wg_desc_sw128(bbase + kk * 2048, Cpad * 128, 1024);
           const uint32_t acc = kk > 0 ? 1u : 0u;
-          wgmma_m64n64<1, 1>(d0, wg_desc_sw128(ah, Cpad * 128, 1024), dbh, acc);
-          wgmma_m64n64<1, 1>(d1, wg_desc_sw128(ah + Cpad * 128, Cpad * 128, 1024), dbh, acc);
-          wgmma_m64n64<1, 1>(d0, wg_desc_sw128(ah, Cpad * 128, 1024), dbm, 1u);
-          wgmma_m64n64<1, 1>(d1, wg_desc_sw128(ah + Cpad * 128, Cpad * 128, 1024), dbm, 1u);
-          wgmma_m64n64<1, 1>(d0, wg_desc_sw128(am, Cpad * 128, 1024), dbh, 1u);
-          wgmma_m64n64<1, 1>(d1, wg_desc_sw128(am + Cpad * 128, Cpad * 128, 1024), dbh, 1u);
+          wgmma_m64n64<1, 1, WG_F16>(d0, wg_desc_sw128(ah, Cpad * 128, 1024), db, acc);
+          wgmma_m64n64<1, 1, WG_F16>(d1, wg_desc_sw128(ah + Cpad * 128, Cpad * 128, 1024), db, acc);
         }
         const uint64_t dsx = wg_desc_sw128(smem_u32(sx0 + s * T4_SX_BYTES), 2048, 1024);
-        wgmma_m64n64<1, 1>(d0, dqx0, dsx, 1u);
-        wgmma_m64n64<1, 1>(d1, dqx1, dsx, 1u);
+        wgmma_m64n64<1, 1, WG_BF16>(d0, dqx0, dsx, 1u);
+        wgmma_m64n64<1, 1, WG_BF16>(d1, dqx1, dsx, 1u);
         wg_commit();
         wg_wait_all();
         mbar_arrive(&sm.stage_free[s]);                    // my part of the group's reads of the stage is done
@@ -334,17 +335,40 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
     }
 #undef DGCN_T4_FILTER8
     flush();
-    t4_group_sync(g);   // the group's wgmma have completed and nobody of the group flushes any more: its query
-                        // planes and candidate buffer become the work area
+    t4_group_sync(g);   // the group's wgmma have completed, nobody of the group reads its accumulator stage or flushes
+                        // any more: the stage and the candidate buffer become the work area
 
     const float cut = (lk[KP - 1] == 0xFFFFFFFFu) ? INFINITY : __uint_as_float(lk[KP - 1] & 0xFFFFF000u);
     const int C = a.C;
     const float* xtb = t.xt + static_cast<int64_t>(b) * N * C;
     const float* xqp = xtb + static_cast<int64_t>(qg) * C;
     const float smax = __ldg(t.sqmax + b);
-    // |approx - exact fp32| <= eps: see the certificate of knn_tc_kernel
-    const float eps = (2.0f * (3.0518e-5f + (5.0f * Cpad + 8.0f) * 1.1921e-7f)) * sqrtf(sqq * smax) +
+    // |approx - exact fp32| <= eps for the single fp16 product (DESIGN.md 6).  With h = fp16(x) = x + e per channel,
+    // h_i.h_j - x_i.x_j = e_i.x_j + h_i.e_j, so by Cauchy-Schwarz |h_i.h_j - x_i.x_j| <= |e_i| |x_j| + |h_i| |e_j|
+    // <= |e_i| sqrt(smax) + |h_i| sqrt(emax): |e_i| and |h_i| of this query are computed here from its fp32 row, emax
+    // (the cloud's max |e_j|^2) by the prologue; e bounds the error whether or not the MMA flushes subnormal inputs
+    // (tc_f16_err2), and the factor 1 + 2^-9 covers the fp32 roundings of these norms.  Doubled on the key; then the
+    // fp32 accumulation of Cpad exact fp16 products + the 16-row -|x_j|^2/2 block and the Cpad roundings of the exact
+    // FMA chain (2^-23 each on |x_i||x_j|), the -|x_j|^2/2 terms and the final additions (2^-20 (|x_i|^2 + smax)).
+    // Valid while no |x_c| exceeds the fp16 range, i.e. below the guard smax < 2^30 (|x_c| < 2^15).
+    float ei2 = 0.f, hi2 = 0.f;
+#pragma unroll 1
+    for (int c = 0; c < C; c += 8) {
+      float v8[8];
+      ldg_f8(xqp + c, v8);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float h = __half2float(tc_to_f16(v8[i]));
+        ei2 += tc_f16_err2(v8[i]);
+        hi2 = fmaf(h, h, hi2);
+      }
+    }
+    const float emax = __ldg(t.sqmax + a.B + b);
+    const float eps = 2.0f * ((sqrtf(ei2) * sqrtf(smax) + sqrtf(hi2) * sqrtf(emax)) * 1.001953125f +
+                              (2.0f * Cpad + 16.0f) * 1.1921e-7f * sqrtf(sqq * smax)) +
                       9.537e-7f * (sqq + smax);
+    // a cloud with some |x_c| >= 2^15 may have been clamped to the fp16 range: no query of it is certified
+    const bool in_range = smax < 1073741824.0f;
     int* sel = reinterpret_cast<int*>(cbuf0 + g * T4_CBUF_BYTES);
     const int sel_ld = tc_sel_ld(a.k);
     // The consumer reduces over the SET of the K nearest (max over neighbours) when every rank is kept and nobody
@@ -361,8 +385,8 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
       // candidates (certainly IN), every entry - and every unlisted candidate, whose approximation is >= cut - above
       // hi = vK + delta(vK) + 2 eps  is beaten by K candidates (certainly OUT).  What lies in [lo, hi] is ranked by
       // the exact key (fp32 FMA chain, ties to the smaller index) and fills the remaining places.
-      constexpr int MB = 12;                                           // band entries a query may hold
-      uint64_t* band = reinterpret_cast<uint64_t*>(qbase + g * T4_QBYTES);   // [MB][TILE] exact keys
+      constexpr int MB = T4_MB;
+      uint64_t* band = reinterpret_cast<uint64_t*>(accg);               // [MB][TILE] exact keys
       const int K = a.K;
       float vK = INFINITY, vK1 = INFINITY;
 #pragma unroll
@@ -392,6 +416,7 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
         }
       }
       if (nb > MB) ok = false;                                         // a cluster of near ties: exact completion kernel
+      ok = ok && in_range;
       // exact keys of the band, four independent FMA chains at a time; per candidate the chain is
       // acc = fma(x_q[c], x_j[c], acc) for c ascending from acc = 0 - the bits of the fp32 kernel
       const int nbe = ok ? nb : 0;
@@ -443,15 +468,17 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
       cta_epilogue_wide<4, false, true, 10>(a, b, q0, nullptr, sm.ok[g], sel, sel_ld, nullptr, 0, r);
     } else {
     // ---- exact re-rank of the listed candidates (fp32 FMA chain, channels ascending) --------------------------
-    uint64_t* list = reinterpret_cast<uint64_t*>(qbase + g * T4_QBYTES);   // [KP][TILE]
+    uint64_t* list = reinterpret_cast<uint64_t*>(accg);                     // [KP][TILE]
     {
-      // Two halves of KP/2 candidates (register budget of a 9-warp CTA at one CTA per SM).  Channels in chunks of 8 in the outer
-      // loop, candidates in the inner one: KP/2 independent FMA chains in flight; per candidate the chain is
+      // Parts of at most 10 candidates (register budget of a 9-warp CTA at one CTA per SM).  Channels in chunks of 8 in
+      // the outer loop, candidates in the inner one: HN independent FMA chains in flight; per candidate the chain is
       // acc = fma(x_q[c], x_j[c], acc) for c ascending from acc = 0 - the bits of the fp32 kernel.
-      constexpr int HN = KP / 2;
+      constexpr int PARTS = KP > 20 ? 4 : 2;
+      constexpr int HN = KP / PARTS;
+      static_assert(HN * PARTS == KP, "list length");
       int e = 0;
 #pragma unroll
-      for (int half = 0; half < 2; ++half) {
+      for (int half = 0; half < PARTS; ++half) {
         float dex[HN];
 #pragma unroll
         for (int u = 0; u < HN; ++u) dex[u] = 0.f;
@@ -495,7 +522,7 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
     // ---- certificate (thread = query): see knn_tc_kernel -------------------------------------------------------
     {
       const uint64_t kth = list[(a.K - 1) * TILE + r];
-      bool ok = kth != KEY_MAX;
+      bool ok = kth != KEY_MAX && in_range;
       if (ok && cut < INFINITY) {
         const float dk = ordered_to_float(static_cast<uint32_t>(kth >> 32));
         ok = (dk + eps < cut);
@@ -514,8 +541,12 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
   }
 }
 
+// List length of knn_tc4_kernel for K = k * d (0: the kernel does not apply): 20 for K <= 9, 32 for K <= 20, chosen
+// with the count model of tests/test_tc4_fp16_bound_cpu.py: on 12,288 queries of random 64-d clouds both leave none
+// uncertified, a list of 28 for K = 20 leaves 8e-5 (the fp16 pre-filter's band is wider than the bf16 split's).
+inline int knn_tc4_list_len(int K) { return K <= 9 ? 20 : K <= 20 ? 32 : 0; }
 inline bool knn_tc4_list_ok(int kp, int k) {
-  return (kp == 16 || kp == 28) && static_cast<size_t>(TILE) * tc_sel_ld(k) * 4 <= static_cast<size_t>(T4_CBUF_BYTES);
+  return (kp == 20 || kp == 32) && static_cast<size_t>(TILE) * tc_sel_ld(k) * 4 <= static_cast<size_t>(T4_CBUF_BYTES);
 }
 
 template <int KP>

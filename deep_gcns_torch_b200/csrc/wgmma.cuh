@@ -1,4 +1,4 @@
-// Hopper warpgroup MMA (wgmma.mma_async, sm_90a): bf16 x bf16 -> fp32, both operands in shared memory, the
+// Hopper warpgroup MMA (wgmma.mma_async, sm_90a): bf16 x bf16 or fp16 x fp16 -> fp32, both operands in shared memory, the
 // accumulator in the registers of the 128 threads of one warpgroup.
 #pragma once
 #include <stdint.h>
@@ -26,26 +26,35 @@ __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.s
 // every committed wgmma of this warpgroup has completed: accumulators readable, operand memory reusable
 __device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
+// Element type of the A and B operands; the accumulator is fp32 either way, so chains of both types may add into the
+// same fragments.
+enum WgElem : int { WG_BF16 = 0, WG_F16 = 1 };
+
 // D[64 x 64] (+)= A[64 x 16] * B[16 x 64]; TA / TB = 1 for MN-major operands, 0 for K-major.  accumulate = 0
 // overwrites D.
-template <int TA, int TB>
+#define DGCN_WGMMA_M64N64(TYPES)                                                                                   \
+  asm volatile(                                                                                                     \
+      "{\n"                                                                                                         \
+      ".reg .pred p;\n"                                                                                             \
+      "setp.ne.b32 p, %34, 0;\n"                                                                                    \
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32." TYPES " "                                                       \
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                                     \
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "                           \
+      "%32, %33, p, 1, 1, %35, %36;\n"                                                                              \
+      "}\n"                                                                                                         \
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), \
+        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),     \
+        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),    \
+        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])                  \
+      : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB)                                                        \
+      : "memory")
+template <int TA, int TB, int ELEM = WG_BF16>
 __device__ __forceinline__ void wgmma_m64n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %34, 0;\n"
-      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-      "%32, %33, p, 1, 1, %35, %36;\n"
-      "}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
-        "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
-        "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
-        "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(da), "l"(db), "r"(accumulate), "n"(TA), "n"(TB)
-      : "memory");
+  static_assert(ELEM == WG_BF16 || ELEM == WG_F16, "operand type");
+  if constexpr (ELEM == WG_F16) DGCN_WGMMA_M64N64("f16.f16");
+  else DGCN_WGMMA_M64N64("bf16.bf16");
 }
+#undef DGCN_WGMMA_M64N64
 // D[64 x 32] (+)= A[64 x 16] * B[16 x 32]
 template <int TA, int TB>
 __device__ __forceinline__ void wgmma_m64n32(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {

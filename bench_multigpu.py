@@ -193,7 +193,10 @@ def sparse_halo_block(dev, rank, world, layers=112, parity_layers=4, num_nodes=P
     return out
 
 
-def ddp_mrgcn_block(dev, rank, world, global_batch=64, points=1024, k=20):
+def ddp_mrgcn_block(dev, rank, world, global_batch=64, points=1024, k=20, sync_bn=False):
+    """sync_bn: convert the model with nn.SyncBatchNorm.convert_sync_batchnorm, so every BatchNorm normalises over
+    the whole global batch (two small all-reduces per graph convolution, forward and backward, plus torch's own for
+    the tail's norms); otherwise each replica normalises over its own shard, as DataParallel does."""
     from bench_models import MRGCN28
     from deep_gcns_torch_b200.gcn_lib import dense as D
     from torch.nn.parallel import DistributedDataParallel as DDP
@@ -204,8 +207,11 @@ def ddp_mrgcn_block(dev, rank, world, global_batch=64, points=1024, k=20):
 
     per_rank = global_batch // world
     torch.manual_seed(0)
-    model = MRGCN28(D, k=k).to(dev).train()
-    ddp = DDP(model, device_ids=[dev.index], broadcast_buffers=False)      # BN statistics stay per replica (DataParallel)
+    model = MRGCN28(D, k=k)
+    if sync_bn:
+        model = torch.nn.SyncBatchNorm.convert_sync_batchnorm(model)
+    model = model.to(dev).train()
+    ddp = DDP(model, device_ids=[dev.index], broadcast_buffers=False)      # BN running statistics stay per replica
     g = torch.Generator().manual_seed(100 + rank)
     inputs = torch.rand(per_rank, 3, points, 1, generator=g).to(dev)
     labels = torch.randint(0, 40, (per_rank,), generator=g).to(dev)
@@ -239,7 +245,7 @@ def ddp_mrgcn_block(dev, rank, world, global_batch=64, points=1024, k=20):
     allreduce_ms = _time_ms(lambda: dist.all_reduce(flat), 5, sync)
     edges = 28 * global_batch * points * k
     return {"model": "MRGCN-28 (modelnet_cls DeepGCN, conv=mr, k=%d, dilation 1..27), fwd + bwd + SGD, train-mode BN" % k,
-            "global_batch": global_batch, "per_rank_batch": per_rank, "points": points,
+            "sync_bn": bool(sync_bn), "global_batch": global_batch, "per_rank_batch": per_rank, "points": points,
             "step_ms": step_ms, "step_ms_without_allreduce": nosync_ms, "allreduce_ms": allreduce_ms,
             "allreduce_exposed_ms": max(0.0, step_ms - nosync_ms), "grad_bytes": int(local.numel()) * 4,
             "edges_per_s_fwd_bwd": edges / (step_ms * 1e-3), "first_loss": loss0,

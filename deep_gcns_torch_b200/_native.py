@@ -10,6 +10,8 @@ import os
 import threading
 
 import torch
+import torch.distributed as dist
+from torch import nn
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG, "lib", "libdgcn.so")
@@ -68,6 +70,53 @@ class GenconvFusionC(ctypes.Structure):
                 ("row_list", ctypes.c_void_p), ("n_rows", c_i64)]
 
 
+ERR_REDUCE = -5            # dgcn_status: the dgcn_bn_sync reduce callback failed
+REDUCE_FN = ctypes.CFUNCTYPE(c_i32, ctypes.c_void_p)
+
+
+class BnSyncC(ctypes.Structure):
+    _fields_ = [("moments", ctypes.c_void_p), ("reduce", REDUCE_FN), ("user", ctypes.c_void_p)]
+
+
+def sync_group(bn):
+    """The process group whose ranks share `bn`'s batch statistics, or None for local statistics: the rule of
+    torch.nn.SyncBatchNorm.forward (batch statistics in training mode, torch.distributed initialised, more than
+    one rank in bn.process_group or, when that is None, in WORLD).  A plain BatchNorm2d never syncs."""
+    if not isinstance(bn, nn.SyncBatchNorm):
+        return None
+    bn_training = bn.training or (bn.running_mean is None and bn.running_var is None)
+    if not (bn_training and bn.training and dist.is_available() and dist.is_initialized()):
+        return None
+    group = bn.process_group or dist.group.WORLD
+    return group if dist.get_world_size(group) > 1 else None
+
+
+class _BnSync:
+    """dgcn_bn_sync of one call: an fp64 moments buffer (2*C_out + 1) and a reduce callback that all-reduces it over
+    `group` on the current stream.  The callback object lives as long as this instance; no exception crosses the C
+    ABI: the callback stores it and returns 1, and check() raises it as the cause."""
+
+    def __init__(self, group, c_out, dev):
+        self.moments = torch.empty(2 * c_out + 1, dtype=torch.float64, device=dev)
+        self.error = None
+
+        def reduce(_user):
+            try:
+                dist.all_reduce(self.moments, group=group)
+                return 0
+            except BaseException as e:     # noqa: B036 - nothing may unwind through the C frames
+                self.error = e
+                return 1
+        self._fn = REDUCE_FN(reduce)
+        self.c = BnSyncC(_ptr(self.moments), self._fn, None)
+
+    def check(self, rc, what):
+        if rc == ERR_REDUCE:
+            raise RuntimeError("%s failed: all-reduce of the BatchNorm statistics raised %r" % (what, self.error)) \
+                from self.error
+        _check(rc, what)
+
+
 _lib = None
 _lock = threading.Lock()
 
@@ -97,6 +146,18 @@ def _declare(lib):
     lib.dgcn_dyn_conv_forward_fused.argtypes = [c_i32, vp, c_i64, c_i64, c_i64, c_i64, c_i64, ctypes.POINTER(DilationC),
                                                 ctypes.POINTER(BasicConvC), c_i64, vp, vp, ctypes.POINTER(BlockFusionC),
                                                 vp, sz, vp]
+    lib.dgcn_graph_conv_forward_sync.restype = ctypes.c_int
+    lib.dgcn_graph_conv_forward_sync.argtypes = [c_i32, vp, c_i64, c_i64, c_i64, c_i64, c_i64, vp, vp, c_i64,
+                                                 ctypes.POINTER(BasicConvC), c_i64, vp, ctypes.POINTER(BnSyncC), vp, sz,
+                                                 vp]
+    lib.dgcn_dyn_conv_forward_sync.restype = ctypes.c_int
+    lib.dgcn_dyn_conv_forward_sync.argtypes = [c_i32, vp, c_i64, c_i64, c_i64, c_i64, c_i64, ctypes.POINTER(DilationC),
+                                               ctypes.POINTER(BasicConvC), c_i64, vp, vp, ctypes.POINTER(BnSyncC), vp,
+                                               sz, vp]
+    lib.dgcn_graph_conv_backward_sync.restype = ctypes.c_int
+    lib.dgcn_graph_conv_backward_sync.argtypes = [c_i32, vp, c_i64, c_i64, c_i64, c_i64, c_i64, vp, vp, c_i64,
+                                                  ctypes.POINTER(BasicConvC), c_i64, vp, vp, vp, vp, vp, vp, vp,
+                                                  ctypes.POINTER(BnSyncC), vp, sz, vp]
     lib.dgcn_graph_conv_backward_workspace_bytes.restype = sz
     lib.dgcn_graph_conv_backward_workspace_bytes.argtypes = [c_i32] + [c_i64] * 5
     lib.dgcn_graph_conv_backward.restype = ctypes.c_int
@@ -214,10 +275,13 @@ def _f32(t):
 
 
 class ConvParams:
-    """Tensors of one BasicConv([2*C_in, C_out]) (gcn_lib/dense/torch_nn.py:48-58)."""
+    """Tensors of one BasicConv([2*C_in, C_out]) (gcn_lib/dense/torch_nn.py:48-58).
+
+    sync_group: process group over which train-mode statistics are shared (SyncBatchNorm), None for local ones.
+    After a synced forward, `moments` holds the cross-rank [sum | sum of squares | count] (fp64, on the device)."""
 
     def __init__(self, weight, bias=None, act="relu", prelu_weight=None, norm=NORM_NONE, bn_weight=None,
-                 bn_bias=None, bn_mean=None, bn_var=None, bn_eps=1e-5):
+                 bn_bias=None, bn_mean=None, bn_var=None, bn_eps=1e-5, sync_group=None):
         self.weight = _f32(weight).reshape(weight.shape[0], -1)
         self.bias = _f32(bias)
         self.act = ACT[act.lower() if isinstance(act, str) else act]
@@ -227,6 +291,14 @@ class ConvParams:
         self.bn_mean, self.bn_var = _f32(bn_mean), _f32(bn_var)
         self.bn_eps = float(bn_eps)
         self.batch_mean = self.batch_var = None
+        self.sync_group = sync_group if norm == NORM_BATCH_TRAIN else None
+        self.moments = None
+
+    def bn_sync(self, dev):
+        """_BnSync for one forward or backward call, or None on the local-statistics path."""
+        if self.sync_group is None:
+            return None
+        return _BnSync(self.sync_group, self.weight.shape[0], dev)
 
     def tensors(self):
         return (self.weight, self.bias, self.prelu_weight, self.bn_weight, self.bn_bias, self.bn_mean, self.bn_var)
@@ -285,9 +357,17 @@ def graph_conv_forward(conv, x, prm, edge_index=None, nbr=None):
         cs = prm.c_struct(dev)
         out = torch.empty((B, c_out, N, 1), dtype=torch.float32, device=dev)
         ws = _workspace(l.dgcn_graph_conv_workspace_bytes(CONV[conv], B, C, c_out, N, k), dev)
-        rc = l.dgcn_graph_conv_forward(CONV[conv], _ptr(x3), B, C, N, sb, sc, _ptr(edge_index), _ptr(nbr), k,
-                                       ctypes.byref(cs), c_out, _ptr(out), _ptr(ws), ws.numel(), _stream(dev))
-        _check(rc, "dgcn_graph_conv_forward")
+        bs = prm.bn_sync(dev)
+        if bs is None:
+            rc = l.dgcn_graph_conv_forward(CONV[conv], _ptr(x3), B, C, N, sb, sc, _ptr(edge_index), _ptr(nbr), k,
+                                           ctypes.byref(cs), c_out, _ptr(out), _ptr(ws), ws.numel(), _stream(dev))
+            _check(rc, "dgcn_graph_conv_forward")
+        else:
+            rc = l.dgcn_graph_conv_forward_sync(CONV[conv], _ptr(x3), B, C, N, sb, sc, _ptr(edge_index), _ptr(nbr), k,
+                                                ctypes.byref(cs), c_out, _ptr(out), ctypes.byref(bs.c), _ptr(ws),
+                                                ws.numel(), _stream(dev))
+            bs.check(rc, "dgcn_graph_conv_forward_sync")
+            prm.moments = bs.moments
     return out
 
 
@@ -324,10 +404,21 @@ def dyn_conv_forward(conv, x, prm, k, dilation=1, cols=None, want_nbr=False, res
             out = torch.empty((B, c_out, N, 1), dtype=torch.float32, device=dev)
         nbr = torch.empty((B, N, k), dtype=torch.int32, device=dev) if want_nbr else None
         ws = _workspace(l.dgcn_dyn_conv_workspace_bytes(CONV[conv], B, C, c_out, N, K), dev)
-        rc = l.dgcn_dyn_conv_forward_fused(CONV[conv], _ptr(x3), B, C, N, sb, sc, ctypes.byref(dil), ctypes.byref(cs),
-                                           c_out, _ptr(out), _ptr(nbr), ctypes.byref(fus) if fus is not None else None,
-                                           _ptr(ws), ws.numel(), _stream(dev))
-        _check(rc, "dgcn_dyn_conv_forward")
+        bs = prm.bn_sync(dev)
+        if bs is None:
+            rc = l.dgcn_dyn_conv_forward_fused(CONV[conv], _ptr(x3), B, C, N, sb, sc, ctypes.byref(dil),
+                                               ctypes.byref(cs), c_out, _ptr(out), _ptr(nbr),
+                                               ctypes.byref(fus) if fus is not None else None, _ptr(ws), ws.numel(),
+                                               _stream(dev))
+            _check(rc, "dgcn_dyn_conv_forward")
+        else:
+            if fus is not None:
+                raise RuntimeError("dyn_conv_forward: the block epilogue does not run with train-mode BatchNorm")
+            rc = l.dgcn_dyn_conv_forward_sync(CONV[conv], _ptr(x3), B, C, N, sb, sc, ctypes.byref(dil),
+                                              ctypes.byref(cs), c_out, _ptr(out), _ptr(nbr), ctypes.byref(bs.c),
+                                              _ptr(ws), ws.numel(), _stream(dev))
+            bs.check(rc, "dgcn_dyn_conv_forward_sync")
+            prm.moments = bs.moments
     return out, nbr
 
 
@@ -362,11 +453,19 @@ def graph_conv_backward(conv, x, prm, grad_out, edge_index=None, nbr=None, need_
              "bn_bias": f(c_out) if prm.norm != NORM_NONE else None,
              "prelu": f(1) if prm.prelu_weight is not None else None}
         ws = _workspace(l.dgcn_graph_conv_backward_workspace_bytes(CONV[conv], B, C, c_out, N, k), dev)
-        rc = l.dgcn_graph_conv_backward(CONV[conv], _ptr(x3), B, C, N, sb, sc, _ptr(edge_index), _ptr(nbr), k,
-                                        ctypes.byref(cs), c_out, _ptr(go), _ptr(g["x"]), _ptr(g["weight"]),
-                                        _ptr(g["bias"]), _ptr(g["bn_weight"]), _ptr(g["bn_bias"]), _ptr(g["prelu"]),
-                                        _ptr(ws), ws.numel(), _stream(dev))
-        _check(rc, "dgcn_graph_conv_backward")
+        bs = prm.bn_sync(dev)
+        grads = (_ptr(g["x"]), _ptr(g["weight"]), _ptr(g["bias"]), _ptr(g["bn_weight"]), _ptr(g["bn_bias"]),
+                 _ptr(g["prelu"]))
+        if bs is None:
+            rc = l.dgcn_graph_conv_backward(CONV[conv], _ptr(x3), B, C, N, sb, sc, _ptr(edge_index), _ptr(nbr), k,
+                                            ctypes.byref(cs), c_out, _ptr(go), *grads, _ptr(ws), ws.numel(),
+                                            _stream(dev))
+            _check(rc, "dgcn_graph_conv_backward")
+        else:       # dx from the cross-rank sums; the parameter gradients stay local (SyncBatchNorm)
+            rc = l.dgcn_graph_conv_backward_sync(CONV[conv], _ptr(x3), B, C, N, sb, sc, _ptr(edge_index), _ptr(nbr), k,
+                                                 ctypes.byref(cs), c_out, _ptr(go), *grads, ctypes.byref(bs.c),
+                                                 _ptr(ws), ws.numel(), _stream(dev))
+            bs.check(rc, "dgcn_graph_conv_backward_sync")
     return g
 
 

@@ -33,7 +33,7 @@ struct EdgeBwdArgs {
   const float* bn_w; const float* bn_m; const float* bn_v; float bn_eps;   // mean/var: running (eval) or batch (train)
   const float* gout;          // (B,co,N)
   const float* sums;          // train pass B: [2][co] = dbeta, dgamma (finalised)
-  double inv_count;           // 1 / (B*N*k)
+  double inv_count;           // 1 / (B*N*k); 1 with synced statistics (sums already divided by the global count)
   float* dpq;                 // (B,2co,N) channel-major, zero-initialised, atomically accumulated
   float* partial;             // [n_cta][3][co]: sum g, sum g*ahat, sum dslope
 };
@@ -143,6 +143,43 @@ __global__ void reduce_partials_kernel(const float* __restrict__ partial, int64_
     __syncthreads();
   }
   if (threadIdx.x == 0) sums[q * C + c] = r[0];
+}
+
+__global__ void store_count_kernel(double* __restrict__ dst, double count) { *dst = count; }
+
+// Synced BatchNorm statistics (dgcn_bn_sync), forward and backward: sync->moments = [the fixed-order fp64 sums of
+// rows q = 0, 1 of the [np][nq][C] partials | count], then the caller enqueues their cross-rank sum on `stream`.
+int bn_sync_moments(const float* partial, int64_t np, int nq, int C, double count, const dgcn_bn_sync* sync,
+                    cudaStream_t stream) {
+  reduce_partials_kernel<<<dim3(C, 2), 256, 0, stream>>>(partial, np, nq, C, sync->moments);
+  DGCN_LAUNCH_CHECK();
+  store_count_kernel<<<1, 1, 0, stream>>>(sync->moments + 2 * static_cast<int64_t>(C), count);
+  DGCN_LAUNCH_CHECK();
+  return sync->reduce(sync->user) == 0 ? DGCN_OK : DGCN_ERR_REDUCE;
+}
+
+// Synced backward: the pass-1 operand [sum g | sum g*ahat] / count from the cross-rank moments, so pass 1 runs with
+// inv_count = 1 and the global count never visits the host.
+__global__ void moments_over_count_kernel(const double* __restrict__ moments, int C, double* __restrict__ sums) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < 2 * C) sums[i] = moments[i] / moments[2 * C];
+}
+
+// Train mode, after pass 0 wrote its partials: sums[0..2C) = (sum g, sum g*ahat) of this rank, with *inv_count
+// left as is, or with sync the global sums already divided by the global count and *inv_count = 1.
+static int bn_bwd_pass0_sums(const float* partial, int64_t np, int C, double count, const dgcn_bn_sync* sync,
+                             double* sums, double* inv_count, cudaStream_t stream) {
+  if (!sync) {
+    reduce_partials_kernel<<<dim3(C, 3), 256, 0, stream>>>(partial, np, 3, C, sums);
+    DGCN_LAUNCH_CHECK();
+    return DGCN_OK;
+  }
+  int rc = bn_sync_moments(partial, np, 3, C, count, sync, stream);
+  if (rc != DGCN_OK) return rc;
+  moments_over_count_kernel<<<static_cast<unsigned>(ceil_div(2 * C, 128)), 128, 0, stream>>>(sync->moments, C, sums);
+  DGCN_LAUNCH_CHECK();
+  *inv_count = 1.0;
+  return DGCN_OK;
 }
 
 // gradients of the BN affine parameters and of the PReLU slope from the reduced sums
@@ -292,7 +329,7 @@ struct MrBnArgs {
   float* z; const float* gout; int B, co, N;
   float slope; const float* prelu; int norm;
   const float* bn_w; const float* bn_m; const float* bn_v; float bn_eps;
-  const double* sums; double inv_count; float* partial;   // [n_cta][3][co]
+  const double* sums; double inv_count; float* partial;   // inv_count as in EdgeBwdArgs; partial [n_cta][3][co]
 };
 template <int PASS>
 __global__ void __launch_bounds__(256) mr_bn_bwd_kernel(const MrBnArgs g) {
@@ -405,16 +442,29 @@ int dgcn_graph_conv_backward(int32_t conv, const float* x, int64_t B, int64_t ci
                              int64_t co, const float* grad_out, float* grad_x, float* grad_weight, float* grad_bias,
                              float* grad_bn_weight, float* grad_bn_bias, float* grad_prelu, void* wsp, size_t ws_bytes,
                              dgcn_stream_t stream_) {
+  return dgcn_graph_conv_backward_sync(conv, x, B, ci, N, sb, sc, edge_index, nbr, k, p, co, grad_out, grad_x,
+                                       grad_weight, grad_bias, grad_bn_weight, grad_bn_bias, grad_prelu, nullptr, wsp,
+                                       ws_bytes, stream_);
+}
+
+int dgcn_graph_conv_backward_sync(int32_t conv, const float* x, int64_t B, int64_t ci, int64_t N, int64_t sb,
+                                  int64_t sc, const int64_t* edge_index, const int32_t* nbr, int64_t k,
+                                  const dgcn_basic_conv* p, int64_t co, const float* grad_out, float* grad_x,
+                                  float* grad_weight, float* grad_bias, float* grad_bn_weight, float* grad_bn_bias,
+                                  float* grad_prelu, const dgcn_bn_sync* sync, void* wsp, size_t ws_bytes,
+                                  dgcn_stream_t stream_) {
   if (conv != DGCN_CONV_EDGE && conv != DGCN_CONV_MR) return DGCN_ERR_UNSUPPORTED;
   if (!x || !p || !p->weight || !grad_out || (!edge_index && !nbr) || B <= 0 || ci <= 0 || co <= 0 || N <= 0 || k <= 0)
     return DGCN_ERR_BAD_ARG;
   if (p->norm != DGCN_NORM_NONE && (!p->bn_mean || !p->bn_var)) return DGCN_ERR_BAD_ARG;
+  if (sync && (!sync->moments || !sync->reduce)) return DGCN_ERR_BAD_ARG;
   if (B > 65535 || co > 65535) return DGCN_ERR_UNSUPPORTED;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   Workspace ws(wsp, ws_bytes);
   BwdPlan pl = bwd_plan(conv, B, ci, co, N);
   const int vec = ((reinterpret_cast<uintptr_t>(x) & 15) == 0 && sb % 4 == 0 && sc % 4 == 0 && N % 4 == 0) ? 1 : 0;
   const bool train = p->norm == DGCN_NORM_BATCH_TRAIN;
+  if (!train) sync = nullptr;
   const float slope = act_slope_of(p);
   const float* prelu = p->act == DGCN_ACT_PRELU ? p->prelu_weight : nullptr;
   float* wk = ws.take<float>(pl.wk);
@@ -444,13 +494,14 @@ int dgcn_graph_conv_backward(int32_t conv, const float* x, int64_t B, int64_t ci
     g.gout = grad_out; g.sums = nullptr; g.inv_count = 1.0 / (static_cast<double>(B) * N * k);
     g.dpq = dpq; g.partial = partial;
     const dim3 grid(ceil_div(N, 32), B);
+    EdgeBwdArgs g1 = g;
     if (train) {
       edge_bwd_kernel<0><<<grid, 256, 0, stream>>>(g);
       DGCN_LAUNCH_CHECK();
-      reduce_partials_kernel<<<dim3(ico, 3), 256, 0, stream>>>(partial, pl.n_partial, 3, ico, sums);
-      DGCN_LAUNCH_CHECK();
+      int rc = bn_bwd_pass0_sums(partial, pl.n_partial, ico, static_cast<double>(B) * N * k, sync, sums, &g1.inv_count,
+                                 stream);
+      if (rc != DGCN_OK) return rc;
     }
-    EdgeBwdArgs g1 = g;
     if (train) {
       // pass B wants (dbeta, dgamma) as float[2][co]: finish_param_grads_kernel does the conversion
       float* sf = ws.take<float>(pl.sf);
@@ -538,8 +589,8 @@ int dgcn_graph_conv_backward(int32_t conv, const float* x, int64_t B, int64_t ci
   if (train) {
     mr_bn_bwd_kernel<0><<<bgrid, 256, 0, stream>>>(mb);
     DGCN_LAUNCH_CHECK();
-    reduce_partials_kernel<<<dim3(ico, 3), 256, 0, stream>>>(partial, pl.n_partial, 3, ico, sums);
-    DGCN_LAUNCH_CHECK();
+    int rc = bn_bwd_pass0_sums(partial, pl.n_partial, ico, static_cast<double>(B) * N, sync, sums, &mb.inv_count, stream);
+    if (rc != DGCN_OK) return rc;
   }
   mr_bn_bwd_kernel<1><<<bgrid, 256, 0, stream>>>(mb);   // z now holds dz
   DGCN_LAUNCH_CHECK();

@@ -506,9 +506,25 @@ __global__ void __launch_bounds__(NTHREADS, 2) mr_node_kernel(const MrNodeArgs g
   }
 }
 
-// Batch statistics from partial sums (fixed order, fp64) -> (scale, shift) and the
-// batch mean / biased variance the host needs for the running-stat update
-// (torch BatchNorm2d training semantics: normalise with biased variance).
+// Channel c's (sum a, sum a^2) over `count` positions -> (scale, shift) and the batch mean / biased
+// variance the host needs for the running-stat update (torch BatchNorm2d training semantics: normalise
+// with biased variance).
+__device__ __forceinline__ void bn_finalize_channel(double s1, double s2, double count, int C, int c,
+                                                    const float* __restrict__ bn_w, const float* __restrict__ bn_b,
+                                                    float eps, float* __restrict__ st, float* __restrict__ mean_out,
+                                                    float* __restrict__ var_out) {
+  double mean = s1 / count;
+  double var = s2 / count - mean * mean;
+  if (var < 0.0) var = 0.0;
+  float inv = 1.0f / sqrtf(static_cast<float>(var) + eps);
+  float s = (bn_w ? bn_w[c] : 1.f) * inv;
+  st[c] = s;
+  st[C + c] = (bn_b ? bn_b[c] : 0.f) - static_cast<float>(mean) * s;
+  if (mean_out) mean_out[c] = static_cast<float>(mean);
+  if (var_out) var_out[c] = static_cast<float>(var);
+}
+
+// Batch statistics from partial sums (fixed order, fp64), one CTA per channel.
 __global__ void bn_finalize_kernel(const float* __restrict__ partial, int64_t np, int C, double count,
                                    const float* __restrict__ bn_w, const float* __restrict__ bn_b, float eps,
                                    float* __restrict__ st, float* __restrict__ mean_out,
@@ -530,18 +546,38 @@ __global__ void bn_finalize_kernel(const float* __restrict__ partial, int64_t np
     }
     __syncthreads();
   }
-  if (threadIdx.x == 0) {
-    double mean = r1[0] / count;
-    double var = r2[0] / count - mean * mean;
-    if (var < 0.0) var = 0.0;
-    float inv = 1.0f / sqrtf(static_cast<float>(var) + eps);
-    float s = (bn_w ? bn_w[c] : 1.f) * inv;
-    st[c] = s;
-    st[C + c] = (bn_b ? bn_b[c] : 0.f) - static_cast<float>(mean) * s;
-    if (mean_out) mean_out[c] = static_cast<float>(mean);
-    if (var_out) var_out[c] = static_cast<float>(var);
-  }
+  if (threadIdx.x == 0) bn_finalize_channel(r1[0], r2[0], count, C, c, bn_w, bn_b, eps, st, mean_out, var_out);
 }
+// Synced statistics (dgcn_bn_sync): the same finalisation from the cross-rank moments [sum a | sum a^2 | count],
+// the count read on the device.
+__global__ void bn_finalize_moments_kernel(const double* __restrict__ moments, int C, const float* __restrict__ bn_w,
+                                           const float* __restrict__ bn_b, float eps, float* __restrict__ st,
+                                           float* __restrict__ mean_out, float* __restrict__ var_out) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c < C) bn_finalize_channel(moments[c], moments[C + c], moments[2 * C], C, c, bn_w, bn_b, eps, st, mean_out, var_out);
+}
+int bn_sync_moments(const float* partial, int64_t np, int nq, int C, double count, const dgcn_bn_sync* sync,
+                    cudaStream_t stream);   // dense_bwd.cu
+
+// Train mode: (scale, shift) into st from the partial rows of `count` positions; with sync, from the
+// statistics of every rank.
+static int bn_finalize(const float* partial, int64_t np, int64_t co, double count, const dgcn_basic_conv* p,
+                       const dgcn_bn_sync* sync, float* st, cudaStream_t stream) {
+  const int C = static_cast<int>(co);
+  if (!sync) {
+    bn_finalize_kernel<<<static_cast<unsigned>(co), 256, 0, stream>>>(partial, np, C, count, p->bn_weight, p->bn_bias,
+                                                                    p->bn_eps, st, p->batch_mean_out, p->batch_var_out);
+    DGCN_LAUNCH_CHECK();
+    return DGCN_OK;
+  }
+  int rc = bn_sync_moments(partial, np, 2, C, count, sync, stream);
+  if (rc != DGCN_OK) return rc;
+  bn_finalize_moments_kernel<<<static_cast<unsigned>(ceil_div(co, 128)), 128, 0, stream>>>(
+      sync->moments, C, p->bn_weight, p->bn_bias, p->bn_eps, st, p->batch_mean_out, p->batch_var_out);
+  DGCN_LAUNCH_CHECK();
+  return DGCN_OK;
+}
+
 // out = s >= 0 ? s*out + t : s*out_min + t   (out_min may be null: plain affine)
 __global__ void bn_apply_kernel(float* __restrict__ out, const float* __restrict__ out_min,
                                 const float* __restrict__ st, int C, int N, int64_t total) {
@@ -696,7 +732,7 @@ float act_slope_of(const dgcn_basic_conv* p) {
 static int conv_forward(int conv, const float* x, int64_t B, int64_t ci, int64_t N, int64_t sb, int64_t sc,
                         const int64_t* edge_index, const int32_t* nbr, int64_t k, const dgcn_dilation* dil,
                         const dgcn_basic_conv* p, int64_t co, float* out, int32_t* nbr_out, Workspace& ws,
-                        cudaStream_t stream, const dgcn_block_fusion* fus = nullptr) {
+                        cudaStream_t stream, const dgcn_block_fusion* fus, const dgcn_bn_sync* sync) {
   const bool fused = dil != nullptr;
   if (fus) {   // block epilogue: out = conv + residual * scale, out possibly a channel slice of a wider buffer
     if (!fused || p->norm == DGCN_NORM_BATCH_TRAIN) return DGCN_ERR_UNSUPPORTED;
@@ -762,10 +798,8 @@ static int conv_forward(int conv, const float* x, int64_t B, int64_t ci, int64_t
       DGCN_LAUNCH_CHECK();
     }
     if (train) {
-      bn_finalize_kernel<<<static_cast<unsigned>(co), 256, 0, stream>>>(
-          partial, pl.n_partial, static_cast<int>(co), static_cast<double>(B) * N * keep, p->bn_weight, p->bn_bias,
-          p->bn_eps, st, p->batch_mean_out, p->batch_var_out);
-      DGCN_LAUNCH_CHECK();
+      int rc = bn_finalize(partial, pl.n_partial, co, static_cast<double>(B) * N * keep, p, sync, st, stream);
+      if (rc != DGCN_OK) return rc;
       const int64_t total = B * co * N;
       bn_apply_kernel<<<static_cast<unsigned>(ceil_div(total, 256)), 256, 0, stream>>>(
           out, out_min, st, static_cast<int>(co), static_cast<int>(N), total);
@@ -813,10 +847,8 @@ static int conv_forward(int conv, const float* x, int64_t B, int64_t ci, int64_t
   mr_node_kernel<<<dim3(ceil_div(N, TILE), ceil_div(co, TILE), B), NTHREADS, 0, stream>>>(m);
   DGCN_LAUNCH_CHECK();
   if (train) {
-    bn_finalize_kernel<<<static_cast<unsigned>(co), 256, 0, stream>>>(
-        partial, pl.n_partial, static_cast<int>(co), static_cast<double>(B) * N, p->bn_weight, p->bn_bias, p->bn_eps,
-        st, p->batch_mean_out, p->batch_var_out);
-    DGCN_LAUNCH_CHECK();
+    int rc = bn_finalize(partial, pl.n_partial, co, static_cast<double>(B) * N, p, sync, st, stream);
+    if (rc != DGCN_OK) return rc;
     const int64_t total = B * co * N;
     bn_apply_kernel<<<static_cast<unsigned>(ceil_div(total, 256)), 256, 0, stream>>>(
         out, nullptr, st, static_cast<int>(co), static_cast<int>(N), total);
@@ -856,12 +888,21 @@ int dgcn_graph_conv_forward(int32_t conv, const float* x, int64_t B, int64_t C_i
                             int64_t stride_c, const int64_t* edge_index, const int32_t* nbr, int64_t k,
                             const dgcn_basic_conv* p, int64_t C_out, float* out, void* wsp, size_t ws_bytes,
                             dgcn_stream_t stream) {
+  return dgcn_graph_conv_forward_sync(conv, x, B, C_in, N, stride_b, stride_c, edge_index, nbr, k, p, C_out, out,
+                                      nullptr, wsp, ws_bytes, stream);
+}
+
+int dgcn_graph_conv_forward_sync(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N, int64_t stride_b,
+                                 int64_t stride_c, const int64_t* edge_index, const int32_t* nbr, int64_t k,
+                                 const dgcn_basic_conv* p, int64_t C_out, float* out, const dgcn_bn_sync* sync,
+                                 void* wsp, size_t ws_bytes, dgcn_stream_t stream) {
   int rc = check_conv_args(conv, x, B, C_in, N, p, C_out, out);
   if (rc != DGCN_OK) return rc;
   if ((!edge_index && !nbr) || k <= 0) return DGCN_ERR_BAD_ARG;
+  if (sync && (!sync->moments || !sync->reduce)) return DGCN_ERR_BAD_ARG;
   Workspace ws(wsp, ws_bytes);
   return conv_forward(conv, x, B, C_in, N, stride_b, stride_c, edge_index, nbr, k, nullptr, p, C_out, out, nullptr,
-                      ws, static_cast<cudaStream_t>(stream));
+                      ws, static_cast<cudaStream_t>(stream), nullptr, sync);
 }
 
 size_t dgcn_dyn_conv_workspace_bytes(int32_t conv, int64_t B, int64_t C_in, int64_t C_out, int64_t N, int64_t K) {
@@ -871,8 +912,8 @@ size_t dgcn_dyn_conv_workspace_bytes(int32_t conv, int64_t B, int64_t C_in, int6
 int dgcn_dyn_conv_forward(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N, int64_t stride_b,
                           int64_t stride_c, const dgcn_dilation* dil, const dgcn_basic_conv* p, int64_t C_out,
                           float* out, int32_t* nbr_out, void* wsp, size_t ws_bytes, dgcn_stream_t stream) {
-  return dgcn_dyn_conv_forward_fused(conv, x, B, C_in, N, stride_b, stride_c, dil, p, C_out, out, nbr_out, nullptr, wsp,
-                                     ws_bytes, stream);
+  return dgcn_dyn_conv_forward_sync(conv, x, B, C_in, N, stride_b, stride_c, dil, p, C_out, out, nbr_out, nullptr, wsp,
+                                    ws_bytes, stream);
 }
 
 int dgcn_dyn_conv_forward_fused(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N, int64_t stride_b,
@@ -884,7 +925,20 @@ int dgcn_dyn_conv_forward_fused(int32_t conv, const float* x, int64_t B, int64_t
   if (!dil) return DGCN_ERR_BAD_ARG;
   Workspace ws(wsp, ws_bytes);
   return conv_forward(conv, x, B, C_in, N, stride_b, stride_c, nullptr, nullptr, 0, dil, p, C_out, out, nbr_out, ws,
-                      static_cast<cudaStream_t>(stream), fus);
+                      static_cast<cudaStream_t>(stream), fus, nullptr);
+}
+
+int dgcn_dyn_conv_forward_sync(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N, int64_t stride_b,
+                               int64_t stride_c, const dgcn_dilation* dil, const dgcn_basic_conv* p, int64_t C_out,
+                               float* out, int32_t* nbr_out, const dgcn_bn_sync* sync, void* wsp, size_t ws_bytes,
+                               dgcn_stream_t stream) {
+  int rc = check_conv_args(conv, x, B, C_in, N, p, C_out, out);
+  if (rc != DGCN_OK) return rc;
+  if (!dil) return DGCN_ERR_BAD_ARG;
+  if (sync && (!sync->moments || !sync->reduce)) return DGCN_ERR_BAD_ARG;
+  Workspace ws(wsp, ws_bytes);
+  return conv_forward(conv, x, B, C_in, N, stride_b, stride_c, nullptr, nullptr, 0, dil, p, C_out, out, nbr_out, ws,
+                      static_cast<cudaStream_t>(stream), nullptr, sync);
 }
 
 }  // extern "C"

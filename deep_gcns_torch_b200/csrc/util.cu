@@ -114,6 +114,7 @@ const char* dgcn_status_string(int status) {
     case DGCN_ERR_UNSUPPORTED: return "request outside what the sm_90a kernels cover";
     case DGCN_ERR_WORKSPACE: return "workspace too small";
     case DGCN_ERR_CUDA: return "CUDA launch failed";
+    case DGCN_ERR_REDUCE: return "cross-rank reduction of the BatchNorm statistics failed (reduce callback)";
     default: return "unknown status";
   }
 }

@@ -17,7 +17,9 @@ __all__ = ["MRConv2d", "EdgeConv2d", "GraphConv2d", "DynConv2d", "PlainDynBlock2
 
 
 class _GraphConvFn(torch.autograd.Function):
-    """autograd node around the fused forward; backward = dgcn_graph_conv_backward."""
+    """autograd node around the fused forward; backward = dgcn_graph_conv_backward.  ctx.prm carries the
+    SyncBatchNorm process group (prm.sync_group) to backward, whose all-reduce then runs in the same order on
+    every rank."""
 
     @staticmethod
     def forward(ctx, owner, x, edge_index, fused, *params):
@@ -60,7 +62,7 @@ class _DenseGraphConv(nn.Module):
                 act = "leakyrelu"
             elif isinstance(m, nn.PReLU):
                 act, prelu = "prelu", m.weight
-            elif isinstance(m, nn.BatchNorm2d):
+            elif isinstance(m, (nn.BatchNorm2d, nn.SyncBatchNorm)):    # (convert_sync_batchnorm)
                 bn = m
         return conv, act, prelu, bn
 
@@ -72,20 +74,25 @@ class _DenseGraphConv(nn.Module):
             use_batch = self.training or bn.running_mean is None
             norm = _native.NORM_BATCH_TRAIN if use_batch else _native.NORM_BATCH_EVAL
             kw = dict(bn_weight=bn.weight, bn_bias=bn.bias, bn_mean=bn.running_mean, bn_var=bn.running_var,
-                      bn_eps=bn.eps)
+                      bn_eps=bn.eps, sync_group=_native.sync_group(bn))
         return _native.ConvParams(conv.weight, conv.bias, act, prelu, norm, **kw)
 
     def _after_forward(self, prm, x, out, k):
         """BatchNorm2d training bookkeeping (running statistics, momentum, unbiased
-        variance, num_batches_tracked) exactly as torch does it."""
+        variance, num_batches_tracked) exactly as torch does it.  With synced statistics the
+        variance is unbiased with the global count, read on the device."""
         bn = self._parts()[3]
         if bn is None or prm.norm != _native.NORM_BATCH_TRAIN or not bn.track_running_stats:
             return
-        count = x.shape[0] * x.shape[2] * (k if self._conv == "edge" else 1)
         with torch.no_grad():
             bn.num_batches_tracked += 1
             mom = bn.momentum if bn.momentum is not None else 1.0 / float(bn.num_batches_tracked)
-            unbiased = prm.batch_var * (count / max(count - 1, 1))
+            if prm.moments is not None:
+                count = prm.moments[-1]
+                unbiased = prm.batch_var * (count / (count - 1).clamp_min(1)).float()
+            else:
+                count = x.shape[0] * x.shape[2] * (k if self._conv == "edge" else 1)
+                unbiased = prm.batch_var * (count / max(count - 1, 1))
             bn.running_mean.mul_(1 - mom).add_(prm.batch_mean, alpha=mom)
             bn.running_var.mul_(1 - mom).add_(unbiased, alpha=mom)
 

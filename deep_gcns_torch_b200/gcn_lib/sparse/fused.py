@@ -49,9 +49,11 @@ def bn_eval_affine(norm):
 
 
 def fusable(conv, norm, h):
-    """The fused kernels cover: no autograd, eval-mode BatchNorm1d with running statistics, GENConv whose MLP
-    is a single Linear (mlp_layers = 1) and no edge features."""
-    return (not torch.is_grad_enabled() and isinstance(norm, nn.BatchNorm1d) and not norm.training and
+    """The fused kernels cover: no autograd, eval-mode BatchNorm1d (or the SyncBatchNorm that
+    convert_sync_batchnorm made of it, on (N, C) rows) with running statistics, GENConv whose MLP is a single
+    Linear (mlp_layers = 1) and no edge features."""
+    is_bn = isinstance(norm, nn.BatchNorm1d) or (isinstance(norm, nn.SyncBatchNorm) and h.dim() == 2)
+    return (not torch.is_grad_enabled() and is_bn and not norm.training and
             norm.running_var is not None and len(conv.mlp) == 1 and isinstance(conv.mlp[0], nn.Linear) and
             not conv.encode_edge and h.is_cuda and h.dtype == torch.float32 and h.shape[1] % 4 == 0 and
             h.shape[1] <= 512)

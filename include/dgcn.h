@@ -35,7 +35,8 @@ enum dgcn_status {
   DGCN_ERR_BAD_ARG = -1,      /* null pointer / negative or inconsistent size */
   DGCN_ERR_UNSUPPORTED = -2,  /* valid request outside what the kernels cover */
   DGCN_ERR_WORKSPACE = -3,    /* workspace too small                          */
-  DGCN_ERR_CUDA = -4          /* launch failed; see dgcn_last_cuda_error()    */
+  DGCN_ERR_CUDA = -4,         /* launch failed; see dgcn_last_cuda_error()    */
+  DGCN_ERR_REDUCE = -5        /* a dgcn_bn_sync reduce callback returned non-zero */
 };
 
 /* gcn_lib/dense/torch_nn.py:9-21 (act_layer) */
@@ -188,6 +189,47 @@ int dgcn_graph_conv_backward(int32_t conv, const float* x, int64_t B, int64_t C_
                              float* grad_x, float* grad_weight, float* grad_bias,
                              float* grad_bn_weight, float* grad_bn_bias, float* grad_prelu,
                              void* ws, size_t ws_bytes, dgcn_stream_t stream);
+
+/* Train-mode BatchNorm statistics shared across data-parallel ranks (torch.nn.SyncBatchNorm).
+ * moments: caller-owned DEVICE buffer of 2*C_out + 1 doubles.  Forward: [sum a | sum a^2 | count] over the
+ *   positions this rank normalises (EdgeConv: the B*N*k edge activations, MRConv: the B*N node activations);
+ *   backward: [sum g | sum g*ahat | count] over the same positions.
+ * reduce(user): called on the calling host thread once per call, after the library has enqueued the LOCAL
+ *   values into `moments` on `stream` and before it enqueues the work that reads them.  It must enqueue the
+ *   element-wise sum of `moments` over all ranks (an all-reduce, in place) in the stream order of `stream` and
+ *   return 0; it must not wait for the device.  Every rank has to make the same sequence of calls, so the
+ *   all-reduces pair up.  A non-zero return abandons the call with DGCN_ERR_REDUCE (work already enqueued
+ *   still runs; the outputs are undefined).
+ * After the reduce the library normalises with the GLOBAL mean and biased variance (forward) and forms grad_x
+ * from the GLOBAL sums and count (backward); the count is read on the device, so ranks may hold different
+ * batch sizes.  The parameter gradients (weight, bias, bn_weight, bn_bias, prelu) stay LOCAL sums, as in
+ * torch.nn.SyncBatchNorm: the data-parallel wrapper averages them.  With the routing of EdgeConv's max fixed
+ * by the sign of the synced scale, the backward must be given the batch statistics its forward returned. */
+typedef struct dgcn_bn_sync {
+  double* moments;
+  int32_t (*reduce)(void* user);
+  void* user;
+} dgcn_bn_sync;
+
+/* dgcn_graph_conv_forward / dgcn_dyn_conv_forward / dgcn_graph_conv_backward with an optional dgcn_bn_sync.
+ * sync == NULL, or a norm other than DGCN_NORM_BATCH_TRAIN: exactly the function without the suffix (same
+ * results, bit for bit, and reduce is never called).  Same workspace sizes as the functions without it. */
+int dgcn_graph_conv_forward_sync(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N,
+                                 int64_t stride_b, int64_t stride_c, const int64_t* edge_index,
+                                 const int32_t* nbr, int64_t k, const dgcn_basic_conv* p,
+                                 int64_t C_out, float* out, const dgcn_bn_sync* sync, void* ws,
+                                 size_t ws_bytes, dgcn_stream_t stream);
+int dgcn_dyn_conv_forward_sync(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N,
+                               int64_t stride_b, int64_t stride_c, const dgcn_dilation* dil,
+                               const dgcn_basic_conv* p, int64_t C_out, float* out, int32_t* nbr_out,
+                               const dgcn_bn_sync* sync, void* ws, size_t ws_bytes, dgcn_stream_t stream);
+int dgcn_graph_conv_backward_sync(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N,
+                                  int64_t stride_b, int64_t stride_c, const int64_t* edge_index,
+                                  const int32_t* nbr, int64_t k,
+                                  const dgcn_basic_conv* p, int64_t C_out, const float* grad_out,
+                                  float* grad_x, float* grad_weight, float* grad_bias,
+                                  float* grad_bn_weight, float* grad_bn_bias, float* grad_prelu,
+                                  const dgcn_bn_sync* sync, void* ws, size_t ws_bytes, dgcn_stream_t stream);
 
 /* ------------------------------------------------------------------------
  * Sparse path

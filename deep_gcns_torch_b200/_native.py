@@ -49,6 +49,11 @@ class CsrHubsC(ctypes.Structure):
                 ("min_degree", c_i32), ("seg_edges", c_i32), ("partial", ctypes.c_void_p)]
 
 
+DTYPE_F32, DTYPE_BF16, DTYPE_F16 = 0, 1, 2     # dgcn_dtype: element type of the rows the sparse kernels read
+_ROW_DTYPE = {torch.float32: DTYPE_F32, torch.bfloat16: DTYPE_BF16, torch.float16: DTYPE_F16}
+HALF_ROWS_MAX_C = 1024     # half rows: the forward's widest channel block; the backward's is ...
+HALF_ROWS_MAX_C_BWD = 512  # ... the fp32 backward's own limit
+
 HUB_MIN_DEGREE = 1024      # rows at least this long are aggregated by CTAs instead of one warp
 HUB_SEG_EDGES = 4096       # ... one CTA per segment of this many edges
 
@@ -194,6 +199,15 @@ def _declare(lib):
     lib.dgcn_debug_tc_certification_read.argtypes = [ctypes.POINTER(c_i64), ctypes.POINTER(c_i64)]
     lib.dgcn_gather_rows.restype = ctypes.c_int
     lib.dgcn_gather_rows.argtypes = [vp, c_i64, vp, c_i64, vp, vp]
+    lib.dgcn_genconv_aggregate_fused_rows.restype = ctypes.c_int
+    lib.dgcn_genconv_aggregate_fused_rows.argtypes = [c_i32, vp, vp, c_i64, c_i64, vp, vp, vp, vp,
+                                                      ctypes.POINTER(GenconvParamsC), ctypes.POINTER(CsrHubsC),
+                                                      ctypes.POINTER(GenconvFusionC), vp, vp]
+    lib.dgcn_genconv_aggregate_backward_rows.restype = ctypes.c_int
+    lib.dgcn_genconv_aggregate_backward_rows.argtypes = [c_i32, vp, vp, c_i64, c_i64, c_i64, vp, vp, vp, vp,
+                                                         ctypes.POINTER(GenconvParamsC), c_i32, vp, vp, vp, vp, vp, vp]
+    lib.dgcn_gather_rows_typed.restype = ctypes.c_int
+    lib.dgcn_gather_rows_typed.argtypes = [c_i32, vp, c_i64, vp, c_i64, vp, vp]
 
 
 def lib():
@@ -272,6 +286,27 @@ def _f32(t):
     if t.dtype != torch.float32 or not t.is_contiguous():
         t = t.float().contiguous()
     return t
+
+
+def aggregate_rows(x_src, x_dst=None, edge_attr=None, pre=None, backward=False):
+    """(dgcn_dtype, x_src, x_dst, edge_attr) as the GENConv aggregate kernels read them.
+
+    bf16 / fp16 rows are read as they are (widened to fp32 in registers: bit for bit the result of the fp32 copy)
+    when x_src is bf16 or fp16, x_dst and edge_attr (where given) have the same dtype, C % 4 == 0,
+    C <= HALF_ROWS_MAX_C (HALF_ROWS_MAX_C_BWD for the backward), no pre-activation is fused and every row base is
+    8-byte aligned.  Non-contiguous half rows are made contiguous in their own dtype.  Everything else gets the
+    fp32 copies it always got."""
+    code = _ROW_DTYPE.get(x_src.dtype)
+    C = x_src.shape[-1]
+    if code not in (None, DTYPE_F32) and pre is None and C % 4 == 0 and \
+            C <= (HALF_ROWS_MAX_C_BWD if backward else HALF_ROWS_MAX_C) and \
+            all(t is None or t.dtype == x_src.dtype for t in (x_dst, edge_attr)):
+        xs = x_src.detach().contiguous()
+        xd = xs if x_dst is x_src else (None if x_dst is None else x_dst.detach().contiguous())
+        ea = None if edge_attr is None else edge_attr.detach().contiguous()
+        if all(t is None or t.data_ptr() % 8 == 0 for t in (xs, xd, ea)):
+            return code, xs, xd, ea
+    return DTYPE_F32, _f32(x_src), _f32(x_dst), _f32(edge_attr)
 
 
 class ConvParams:
@@ -537,7 +572,7 @@ def genconv_aggregate(x_src, x_dst, csr, prm, edge_attr=None, out=None, pre=None
     rows (int32) / skip_hubs: destination rows of this launch (dgcn_genconv_fusion)."""
     rowptr, src, eid = csr[:3]
     _require_cuda(x_src, x_dst, rowptr, src, eid, edge_attr, out, rows)
-    x_src, x_dst, edge_attr = _f32(x_src), _f32(x_dst), _f32(edge_attr)
+    dtype, x_src, x_dst, edge_attr = aggregate_rows(x_src, x_dst, edge_attr, pre=pre)
     N, C = rowptr.numel() - 1, x_src.shape[1]
     dev = x_src.device
     hubs = None
@@ -550,6 +585,8 @@ def genconv_aggregate(x_src, x_dst, csr, prm, edge_attr=None, out=None, pre=None
             out = torch.empty((N, C), dtype=torch.float32, device=dev)
         elif out.shape != (N, C) or out.dtype != torch.float32 or not out.is_contiguous():
             raise RuntimeError("genconv_aggregate: out must be a contiguous fp32 (N, C) tensor")
+        elif dtype != DTYPE_F32 and out.data_ptr() % 16 != 0:       # half rows store out as float4
+            dtype, x_src, x_dst, edge_attr = DTYPE_F32, _f32(x_src), _f32(x_dst), _f32(edge_attr)
         fus, keep = None, None
         if pre is not None or rows is not None or skip_hubs:
             fus = GenconvFusionC()
@@ -563,33 +600,39 @@ def genconv_aggregate(x_src, x_dst, csr, prm, edge_attr=None, out=None, pre=None
                 fus.row_list, fus.n_rows = (rows.data_ptr() or None), rows.numel()
                 if rows.numel() == 0 and skip_hubs:
                     return out
-        rc = lib().dgcn_genconv_aggregate_fused(_ptr(x_src), _ptr(x_dst), N, C, _ptr(rowptr), _ptr(src), _ptr(eid),
-                                                _ptr(edge_attr), ctypes.byref(prm),
-                                                ctypes.byref(hubs) if hubs is not None else None,
-                                                ctypes.byref(fus) if fus is not None else None, _ptr(out),
-                                                _stream(dev))
+        rc = lib().dgcn_genconv_aggregate_fused_rows(dtype, _ptr(x_src), _ptr(x_dst), N, C, _ptr(rowptr), _ptr(src),
+                                                     _ptr(eid), _ptr(edge_attr), ctypes.byref(prm),
+                                                     ctypes.byref(hubs) if hubs is not None else None,
+                                                     ctypes.byref(fus) if fus is not None else None, _ptr(out),
+                                                     _stream(dev))
         _check(rc, "dgcn_genconv_aggregate")
     return out
 
 
 def genconv_aggregate_backward(x_src, x_dst, csr, prm, grad_out, edge_attr=None, softmax_grad=False,
                                need_edge_attr=False):
-    """dgcn_genconv_aggregate_backward: (grad_x_src (N_src,C), grad_x_dst (N,C) | None,
-    grad_edge_attr | None, grad_scalars (4) = d/dt, d/dp, d/dy, d/dmsg_scale)."""
+    """dgcn_genconv_aggregate_backward(_rows): (grad_x_src (N_src,C) fp32, grad_x_dst (N,C) fp32 | None,
+    grad_edge_attr in edge_attr's row dtype | None, grad_scalars (4) = d/dt, d/dp, d/dy, d/dmsg_scale)."""
     rowptr, src, eid = csr[:3]
     _require_cuda(x_src, x_dst, grad_out, edge_attr)
-    x_src, x_dst, edge_attr, grad_out = _f32(x_src), _f32(x_dst), _f32(edge_attr), _f32(grad_out)
+    dtype, x_src, x_dst, edge_attr = aggregate_rows(x_src, x_dst, edge_attr, backward=True)
+    grad_out = _f32(grad_out)
     N, C = rowptr.numel() - 1, x_src.shape[1]
     dev = x_src.device
     with torch.cuda.device(dev):
-        gsrc = torch.zeros_like(x_src)
+        gsrc = torch.zeros(x_src.shape, dtype=torch.float32, device=dev)
         gdst = torch.empty((N, C), dtype=torch.float32, device=dev) if x_dst is not None else None
-        gea = torch.zeros_like(edge_attr) if (need_edge_attr and edge_attr is not None) else None
+        gea = None
+        if need_edge_attr and edge_attr is not None:
+            # half rows: every CSR edge writes its row once (rounded like Tensor.to), so when edge_attr has one row
+            # per edge nothing needs clearing (src keeps >= 1 element; an edgeless graph takes the zeros)
+            full = dtype != DTYPE_F32 and edge_attr.shape[0] == src.numel() and edge_attr.shape[0] > 1
+            gea = torch.empty_like(edge_attr) if full else torch.zeros_like(edge_attr)
         gsc = torch.zeros(4, dtype=torch.float32, device=dev)
-        rc = lib().dgcn_genconv_aggregate_backward(_ptr(x_src), _ptr(x_dst), N, x_src.shape[0], C, _ptr(rowptr),
-                                                   _ptr(src), _ptr(eid), _ptr(edge_attr), ctypes.byref(prm),
-                                                   int(bool(softmax_grad)), _ptr(grad_out), _ptr(gsrc), _ptr(gdst),
-                                                   _ptr(gea), _ptr(gsc), _stream(dev))
+        rc = lib().dgcn_genconv_aggregate_backward_rows(dtype, _ptr(x_src), _ptr(x_dst), N, x_src.shape[0], C,
+                                                        _ptr(rowptr), _ptr(src), _ptr(eid), _ptr(edge_attr),
+                                                        ctypes.byref(prm), int(bool(softmax_grad)), _ptr(grad_out),
+                                                        _ptr(gsrc), _ptr(gdst), _ptr(gea), _ptr(gsc), _stream(dev))
         _check(rc, "dgcn_genconv_aggregate_backward")
     return gsrc, gdst, gea, gsc
 
@@ -621,14 +664,20 @@ def linear_residual(a, weight, bias=None, res=None, out=None):
 
 
 def gather_rows(x, rows, out=None):
+    """out[r] = x[rows[r]] in x's dtype (fp32, bf16 or fp16; other dtypes are copied as fp32)."""
     _require_cuda(x, rows, out)
-    x = _f32(x)
+    dtype = _ROW_DTYPE.get(x.dtype)
+    x = x.detach().contiguous() if dtype is not None else _f32(x)
+    dtype = DTYPE_F32 if dtype is None else dtype
     rows = rows.to(torch.int32).contiguous()
     R, C = rows.numel(), x.shape[1]
     with torch.cuda.device(x.device):
         if out is None:
-            out = torch.empty((R, C), dtype=torch.float32, device=x.device)
-        _check(lib().dgcn_gather_rows(_ptr(x), C, _ptr(rows), R, _ptr(out), _stream(x.device)), "dgcn_gather_rows")
+            out = torch.empty((R, C), dtype=x.dtype, device=x.device)
+        elif out.dtype != x.dtype or out.shape != (R, C) or not out.is_contiguous():
+            raise RuntimeError("gather_rows: out must be a contiguous (R, C) tensor of x's dtype")
+        _check(lib().dgcn_gather_rows_typed(dtype, _ptr(x), C, _ptr(rows), R, _ptr(out), _stream(x.device)),
+               "dgcn_gather_rows_typed")
     return out
 
 

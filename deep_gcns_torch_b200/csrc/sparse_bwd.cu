@@ -5,11 +5,16 @@
 // pass A recomputes the row's aggregate (running max / sums), the row-local part (MsgNorm,
 // residual, degree scaling) is differentiated in registers, pass B walks the row's edges again
 // and scatters d(message) to the source rows with atomics.
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
 #include "common.cuh"
 
 namespace dgcn {
 
 struct AggrBwdArgs {
+  // x_src / x_dst / edge_attr / gea hold rows of the kernel's element type T, everything else is fp32; typed float*
+  // so that the fp32 kernels compile exactly as they did before T existed
   const float* x_src; const float* x_dst; int N, C;
   const int32_t* rowptr; const int32_t* src; const int32_t* eid; const float* edge_attr;
   int aggr;
@@ -19,7 +24,17 @@ struct AggrBwdArgs {
   const float* gout; float* gx_src; float* gx_dst; float* gea; float* gscalars;
 };
 
-template <int NCH>   // channels per lane (c = lane + 32*u)
+// one row element, widened exactly to fp32 / rounded to nearest even from fp32 (what Tensor.to does)
+__device__ __forceinline__ float ld_row(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float ld_row(const __nv_bfloat16* p) { return __bfloat162float(__ldg(p)); }
+__device__ __forceinline__ float ld_row(const __half* p) { return __half2float(__ldg(p)); }
+template <typename T> __device__ __forceinline__ T from_f32(float v);
+template <> __device__ __forceinline__ float from_f32<float>(float v) { return v; }
+template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+template <> __device__ __forceinline__ __half from_f32<__half>(float v) { return __float2half_rn(v); }
+
+// T: element type of the rows (float, __nv_bfloat16, __half); NCH: channels per lane (c = lane + 32*u)
+template <typename T, int NCH>
 __global__ void __launch_bounds__(256) genconv_aggregate_bwd_kernel(const AggrBwdArgs g) {
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -48,8 +63,8 @@ __global__ void __launch_bounds__(256) genconv_aggregate_bwd_kernel(const AggrBw
     for (int u = 0; u < NCH; ++u) {
       const int c = lane + 32 * u;
       if (c < C) {
-        float v = __ldg(g.x_src + static_cast<int64_t>(s) * C + c);
-        if (g.edge_attr) v += __ldg(g.edge_attr + static_cast<int64_t>(ei) * C + c);
+        float v = ld_row(reinterpret_cast<const T*>(g.x_src) + static_cast<int64_t>(s) * C + c);
+        if (g.edge_attr) v += ld_row(reinterpret_cast<const T*>(g.edge_attr) + static_cast<int64_t>(ei) * C + c);
         const float msg = g.raw ? v : fmaxf(v, 0.f) + g.eps;
         if (softmax) {
           const float z = msg * t, d = z - M[u], ex = __expf(-fabsf(d));
@@ -98,7 +113,7 @@ __global__ void __launch_bounds__(256) genconv_aggregate_bwd_kernel(const AggrBw
   for (int u = 0; u < NCH; ++u) {
     const int c = lane + 32 * u;
     gh[u] = c < C ? __ldg(g.gout + static_cast<int64_t>(row) * C + c) : 0.f;
-    xr[u] = (need_x && c < C) ? __ldg(g.x_dst + static_cast<int64_t>(row) * C + c) : 0.f;
+    xr[u] = (need_x && c < C) ? ld_row(reinterpret_cast<const T*>(g.x_dst) + static_cast<int64_t>(row) * C + c) : 0.f;
     n2m = fmaf(m[u], m[u], n2m);
     n2x = fmaf(xr[u], xr[u], n2x);
     dot_gm = fmaf(gh[u], m[u], dot_gm);
@@ -164,8 +179,8 @@ __global__ void __launch_bounds__(256) genconv_aggregate_bwd_kernel(const AggrBw
     for (int u = 0; u < NCH; ++u) {
       const int c = lane + 32 * u;
       if (c < C) {
-        float v = __ldg(g.x_src + static_cast<int64_t>(s) * C + c);
-        if (g.edge_attr) v += __ldg(g.edge_attr + static_cast<int64_t>(ei) * C + c);
+        float v = ld_row(reinterpret_cast<const T*>(g.x_src) + static_cast<int64_t>(s) * C + c);
+        if (g.edge_attr) v += ld_row(reinterpret_cast<const T*>(g.edge_attr) + static_cast<int64_t>(ei) * C + c);
         const float msg = g.raw ? v : fmaxf(v, 0.f) + g.eps;
         float dmsg;
         if (softmax) {
@@ -188,7 +203,7 @@ __global__ void __launch_bounds__(256) genconv_aggregate_bwd_kernel(const AggrBw
         }
         const float dv = (g.raw || v > 0.f) ? dmsg : 0.f;
         if (g.gx_src) atomicAdd(g.gx_src + static_cast<int64_t>(s) * C + c, dv);
-        if (g.gea) g.gea[static_cast<int64_t>(ei) * C + c] = dv;
+        if (g.gea) reinterpret_cast<T*>(g.gea)[static_cast<int64_t>(ei) * C + c] = from_f32<T>(dv);
       }
     }
   }
@@ -205,6 +220,16 @@ __global__ void __launch_bounds__(256) genconv_aggregate_bwd_kernel(const AggrBw
   }
 }
 
+template <typename T>
+static void launch_bwd(const AggrBwdArgs& g, cudaStream_t s) {
+  const unsigned grid = static_cast<unsigned>(ceil_div(g.N, 8));
+  if (g.C <= 32) genconv_aggregate_bwd_kernel<T, 1><<<grid, 256, 0, s>>>(g);
+  else if (g.C <= 64) genconv_aggregate_bwd_kernel<T, 2><<<grid, 256, 0, s>>>(g);
+  else if (g.C <= 128) genconv_aggregate_bwd_kernel<T, 4><<<grid, 256, 0, s>>>(g);
+  else if (g.C <= 256) genconv_aggregate_bwd_kernel<T, 8><<<grid, 256, 0, s>>>(g);
+  else genconv_aggregate_bwd_kernel<T, 16><<<grid, 256, 0, s>>>(g);
+}
+
 }  // namespace dgcn
 
 using namespace dgcn;
@@ -215,28 +240,38 @@ extern "C" int dgcn_genconv_aggregate_backward(const float* x_src, const float* 
                                                const dgcn_genconv_params* prm, int32_t softmax_grad,
                                                const float* grad_out, float* grad_x_src, float* grad_x_dst,
                                                float* grad_edge_attr, float* grad_scalars, dgcn_stream_t stream) {
+  return dgcn_genconv_aggregate_backward_rows(DGCN_F32, x_src, x_dst, N, N_src, C, rowptr, src, eid, edge_attr, prm,
+                                              softmax_grad, grad_out, grad_x_src, grad_x_dst, grad_edge_attr,
+                                              grad_scalars, stream);
+}
+
+extern "C" int dgcn_genconv_aggregate_backward_rows(int32_t dtype, const void* x_src, const void* x_dst, int64_t N,
+                                                    int64_t N_src, int64_t C, const int32_t* rowptr,
+                                                    const int32_t* src, const int32_t* eid, const void* edge_attr,
+                                                    const dgcn_genconv_params* prm, int32_t softmax_grad,
+                                                    const float* grad_out, float* grad_x_src, float* grad_x_dst,
+                                                    void* grad_edge_attr, float* grad_scalars, dgcn_stream_t stream) {
   (void)N_src;
   if (!x_src || !rowptr || !src || !prm || !grad_out || N < 0 || C <= 0) return DGCN_ERR_BAD_ARG;
+  if (dtype != DGCN_F32 && dtype != DGCN_BF16 && dtype != DGCN_F16) return DGCN_ERR_BAD_ARG;
   if (!x_dst && (prm->msg_norm || prm->add_residual)) return DGCN_ERR_BAD_ARG;
   if ((edge_attr || grad_edge_attr) && !eid) return DGCN_ERR_BAD_ARG;
   if (prm->aggr < DGCN_AGGR_SOFTMAX || prm->aggr > DGCN_AGGR_MAX) return DGCN_ERR_UNSUPPORTED;
   if (N == 0) return DGCN_OK;
   AggrBwdArgs g{};
-  g.x_src = x_src; g.x_dst = x_dst; g.N = static_cast<int>(N); g.C = static_cast<int>(C);
-  g.rowptr = rowptr; g.src = src; g.eid = eid; g.edge_attr = edge_attr;
+  g.x_src = static_cast<const float*>(x_src); g.x_dst = static_cast<const float*>(x_dst);
+  g.N = static_cast<int>(N); g.C = static_cast<int>(C);
+  g.rowptr = rowptr; g.src = src; g.eid = eid; g.edge_attr = static_cast<const float*>(edge_attr);
   g.aggr = prm->aggr;
   g.t = prm->t; g.t_dev = prm->t_dev; g.p = prm->p; g.p_dev = prm->p_dev; g.y = prm->y; g.y_dev = prm->y_dev;
   g.eps = prm->eps; g.msg_norm = prm->msg_norm; g.msg_scale = prm->msg_scale; g.msg_scale_dev = prm->msg_scale_dev;
   g.add_residual = prm->add_residual; g.raw = prm->raw_message; g.softmax_grad = softmax_grad;
-  g.gout = grad_out; g.gx_src = grad_x_src; g.gx_dst = grad_x_dst; g.gea = grad_edge_attr; g.gscalars = grad_scalars;
+  g.gout = grad_out; g.gx_src = grad_x_src; g.gx_dst = grad_x_dst; g.gea = static_cast<float*>(grad_edge_attr); g.gscalars = grad_scalars;
+  if (C > 512 || (dtype != DGCN_F32 && (C % 4) != 0)) return DGCN_ERR_UNSUPPORTED;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const unsigned grid = static_cast<unsigned>(ceil_div(N, 8));
-  if (C <= 32) genconv_aggregate_bwd_kernel<1><<<grid, 256, 0, s>>>(g);
-  else if (C <= 64) genconv_aggregate_bwd_kernel<2><<<grid, 256, 0, s>>>(g);
-  else if (C <= 128) genconv_aggregate_bwd_kernel<4><<<grid, 256, 0, s>>>(g);
-  else if (C <= 256) genconv_aggregate_bwd_kernel<8><<<grid, 256, 0, s>>>(g);
-  else if (C <= 512) genconv_aggregate_bwd_kernel<16><<<grid, 256, 0, s>>>(g);
-  else return DGCN_ERR_UNSUPPORTED;
+  if (dtype == DGCN_BF16) launch_bwd<__nv_bfloat16>(g, s);
+  else if (dtype == DGCN_F16) launch_bwd<__half>(g, s);
+  else launch_bwd<float>(g, s);
   DGCN_LAUNCH_CHECK();
   return DGCN_OK;
 }

@@ -189,8 +189,8 @@ def start_halo_exchange(part, channels, slot=0, group=None):
 
 
 def halo_exchange(x_local, part, gather=None, group=None):
-    """[local rows | halo rows] as a NEW tensor (simple, allocation per call): packs the rows the peers asked
-    for and swaps them all-to-all.  The persistent-buffer path is start_halo_exchange()."""
+    """[local rows | halo rows] as a NEW tensor in x_local's dtype (simple, allocation per call): packs the rows
+    the peers asked for and swaps them all-to-all.  The persistent-buffer path is start_halo_exchange()."""
     group = group if group is not None else part.group
     send = gather(x_local, part.send_rows) if gather is not None else _pack(x_local, part.send_rows)
     recv = torch.empty((part.n_halo, x_local.shape[1]), dtype=x_local.dtype, device=x_local.device)

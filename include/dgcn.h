@@ -8,7 +8,8 @@
  *
  * Conventions
  *   - all pointers are DEVICE pointers unless the name ends in _host;
- *   - tensors are fp32, dense, in the reference's own layouts:
+ *   - tensors are fp32 (the sparse *_rows / *_typed entry points also take bf16 / fp16
+ *     rows, dgcn_dtype), dense, in the reference's own layouts:
  *       dense path   x (B, C, N, 1)  -> element (b,c,n) at x[b*stride_b + c*stride_c + n]
  *                    edge_index (2, B, N, k) int64, plane 0 = neighbour j, plane 1 = centre i
  *       sparse path  x (N, C) row-major, edge_index (2, E) int64 row 0 = source, row 1 = target
@@ -48,6 +49,9 @@ enum dgcn_act { DGCN_ACT_NONE = 0, DGCN_ACT_RELU = 1, DGCN_ACT_LEAKYRELU = 2, DG
 enum dgcn_norm { DGCN_NORM_NONE = 0, DGCN_NORM_BATCH_EVAL = 1, DGCN_NORM_BATCH_TRAIN = 2 };
 /* gcn_lib/dense/torch_vertex.py:44-49 (GraphConv2d dispatch) */
 enum dgcn_conv { DGCN_CONV_EDGE = 0, DGCN_CONV_MR = 1 };
+/* Element type of the node / edge rows the sparse entry points read (the *_rows / *_typed variants).  bf16 and
+ * fp16 rows are widened to fp32 in registers (exact) and everything is computed in fp32 as for fp32 rows. */
+enum dgcn_dtype { DGCN_F32 = 0, DGCN_BF16 = 1, DGCN_F16 = 2 };
 /* gcn_lib/sparse/torch_message.py:44-85 (GenMessagePassing.aggregate) */
 enum dgcn_aggr {
   DGCN_AGGR_SOFTMAX = 0,     /* 'softmax' and 'softmax_sg' (identical forward) */
@@ -317,6 +321,17 @@ int dgcn_genconv_aggregate_fused(const float* x_src, const float* x_dst, int64_t
                                  const dgcn_csr_hubs* hubs /* may be NULL */,
                                  const dgcn_genconv_fusion* fus /* may be NULL */, float* out,
                                  dgcn_stream_t stream);
+/* The same on rows of element type `dtype` (dgcn_dtype; dgcn_genconv_aggregate_fused = DGCN_F32): x_src, x_dst and
+ * edge_attr are all of that type, out stays fp32.  For DGCN_BF16 / DGCN_F16 the result is bit-identical to the
+ * fp32 call on the same rows converted to fp32.  Half rows need C % 4 == 0, C <= 1024, 8-byte aligned x_src /
+ * x_dst / edge_attr, a 16-byte aligned out and no pre-activation (fus->pre_scale NULL); anything else returns
+ * DGCN_ERR_UNSUPPORTED. */
+int dgcn_genconv_aggregate_fused_rows(int32_t dtype, const void* x_src, const void* x_dst, int64_t N, int64_t C,
+                                      const int32_t* rowptr, const int32_t* src, const int32_t* eid,
+                                      const void* edge_attr, const dgcn_genconv_params* prm,
+                                      const dgcn_csr_hubs* hubs /* may be NULL */,
+                                      const dgcn_genconv_fusion* fus /* may be NULL */, float* out,
+                                      dgcn_stream_t stream);
 
 /* Row-wise Linear with fused bias and skip connection on the tensor cores (wgmma):
  *   out[n][m] = sum_k a[n][k] * weight[m][k] (+ bias[m]) (+ res[n][m])
@@ -345,11 +360,26 @@ int dgcn_genconv_aggregate_backward(const float* x_src, const float* x_dst, int6
                                     int32_t softmax_grad, const float* grad_out,
                                     float* grad_x_src, float* grad_x_dst, float* grad_edge_attr,
                                     float* grad_scalars, dgcn_stream_t stream);
+/* The same on rows of element type `dtype` (dgcn_genconv_aggregate_backward = DGCN_F32): x_src, x_dst, edge_attr
+ * and grad_edge_attr are of that type; grad_out, grad_x_src, grad_x_dst and grad_scalars stay fp32.
+ * grad_edge_attr is written once per CSR edge, rounded to nearest even (no zero-initialisation needed when eid
+ * covers every edge_attr row).  Half rows need C % 4 == 0 and C <= 512; anything else returns
+ * DGCN_ERR_UNSUPPORTED. */
+int dgcn_genconv_aggregate_backward_rows(int32_t dtype, const void* x_src, const void* x_dst, int64_t N,
+                                         int64_t N_src, int64_t C, const int32_t* rowptr,
+                                         const int32_t* src, const int32_t* eid,
+                                         const void* edge_attr, const dgcn_genconv_params* prm,
+                                         int32_t softmax_grad, const float* grad_out,
+                                         float* grad_x_src, float* grad_x_dst, void* grad_edge_attr,
+                                         float* grad_scalars, dgcn_stream_t stream);
 
 /* Halo packing for node-partitioned graphs (new functionality; the reference
  * has no multi-GPU sparse path, SURVEY.md 3.4): out[r,:] = x[rows[r],:]. */
 int dgcn_gather_rows(const float* x, int64_t C, const int32_t* rows, int64_t R, float* out,
                      dgcn_stream_t stream);
+/* The same for rows of element type `dtype` (dgcn_dtype): x and out are of that type, rows are copied as is. */
+int dgcn_gather_rows_typed(int32_t dtype, const void* x, int64_t C, const int32_t* rows, int64_t R, void* out,
+                           dgcn_stream_t stream);
 
 /* ------------------------------------------------------------------------
  * Measurement hook (bench.py): when enabled, the dominant kernel of each path

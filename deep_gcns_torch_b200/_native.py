@@ -75,6 +75,10 @@ class GenconvFusionC(ctypes.Structure):
                 ("row_list", ctypes.c_void_p), ("n_rows", c_i64)]
 
 
+class KeepMaskC(ctypes.Structure):
+    _fields_ = [("keep_bits", ctypes.c_void_p), ("words_per_row", c_i64), ("keep_scale", ctypes.c_float)]
+
+
 ERR_REDUCE = -5            # dgcn_status: the dgcn_bn_sync reduce callback failed
 REDUCE_FN = ctypes.CFUNCTYPE(c_i32, ctypes.c_void_p)
 
@@ -208,6 +212,21 @@ def _declare(lib):
                                                          ctypes.POINTER(GenconvParamsC), c_i32, vp, vp, vp, vp, vp, vp]
     lib.dgcn_gather_rows_typed.restype = ctypes.c_int
     lib.dgcn_gather_rows_typed.argtypes = [c_i32, vp, c_i64, vp, c_i64, vp, vp]
+    lib.dgcn_genconv_aggregate_fused_keep.restype = ctypes.c_int
+    lib.dgcn_genconv_aggregate_fused_keep.argtypes = [c_i32, vp, vp, c_i64, c_i64, vp, vp, vp, vp,
+                                                      ctypes.POINTER(GenconvParamsC), ctypes.POINTER(CsrHubsC),
+                                                      ctypes.POINTER(GenconvFusionC), ctypes.POINTER(KeepMaskC), vp, vp]
+    lib.dgcn_genconv_aggregate_backward_keep.restype = ctypes.c_int
+    lib.dgcn_genconv_aggregate_backward_keep.argtypes = [c_i32, vp, vp, c_i64, c_i64, c_i64, vp, vp, vp, vp,
+                                                         ctypes.POINTER(GenconvParamsC), c_i32, vp, vp, c_i32,
+                                                         ctypes.POINTER(KeepMaskC), vp, vp, vp, vp, vp, vp]
+    lib.dgcn_keep_bits_pack.restype = ctypes.c_int
+    lib.dgcn_keep_bits_pack.argtypes = [vp, c_i64, c_i64, vp, vp]
+    lib.dgcn_res_plus_backward_gy.restype = ctypes.c_int
+    lib.dgcn_res_plus_backward_gy.argtypes = [vp, c_i64, c_i64, vp, vp, ctypes.POINTER(KeepMaskC), vp, vp, vp, vp, vp,
+                                              vp]
+    lib.dgcn_res_plus_backward_dh.restype = ctypes.c_int
+    lib.dgcn_res_plus_backward_dh.argtypes = [vp, vp, c_i64, c_i64, vp, vp, vp, vp, vp, vp]
 
 
 def lib():
@@ -564,15 +583,29 @@ def genconv_params(aggr, t=1.0, p=1.0, y=0.0, eps=1e-7, msg_scale=None, add_resi
     return prm, keep
 
 
-def genconv_aggregate(x_src, x_dst, csr, prm, edge_attr=None, out=None, pre=None, rows=None, skip_hubs=False):
-    """dgcn_genconv_aggregate(_fused): out (N, C) = x_dst + MsgNorm(aggregate(message)).
+def _keep_mask(keep):
+    """keep = (bits (N, W) int32 from keep_bits, keep_scale) -> (dgcn_keep_mask, bits) | (None, None)."""
+    if keep is None:
+        return None, None
+    bits = keep[0]
+    if bits.dtype != torch.int32 or bits.dim() != 2 or not bits.is_contiguous():
+        raise RuntimeError("keep bits must be a contiguous (N, W) int32 tensor (keep_bits)")
+    return KeepMaskC(_ptr(bits), bits.shape[1], float(keep[1])), bits
+
+
+def genconv_aggregate(x_src, x_dst, csr, prm, edge_attr=None, out=None, pre=None, rows=None, skip_hubs=False,
+                      keep=None):
+    """dgcn_genconv_aggregate(_fused / _fused_keep): out (N, C) = x_dst + MsgNorm(aggregate(message)).
 
     out: write into this (N, C) tensor (e.g. a view of a persistent buffer) instead of a new one.
     pre = (scale (C), shift (C), relu): rows of x_src / x_dst are read as act(scale * x + shift).
+    keep = (bits, keep_scale) (dgcn_keep_mask, with pre and relu): rows are read as
+    keep ? relu(scale * x + shift) * keep_scale : 0 (dropout in training).
     rows (int32) / skip_hubs: destination rows of this launch (dgcn_genconv_fusion)."""
     rowptr, src, eid = csr[:3]
-    _require_cuda(x_src, x_dst, rowptr, src, eid, edge_attr, out, rows)
+    _require_cuda(x_src, x_dst, rowptr, src, eid, edge_attr, out, rows, None if keep is None else keep[0])
     dtype, x_src, x_dst, edge_attr = aggregate_rows(x_src, x_dst, edge_attr, pre=pre)
+    km, _bits = _keep_mask(keep)
     N, C = rowptr.numel() - 1, x_src.shape[1]
     dev = x_src.device
     hubs = None
@@ -600,22 +633,28 @@ def genconv_aggregate(x_src, x_dst, csr, prm, edge_attr=None, out=None, pre=None
                 fus.row_list, fus.n_rows = (rows.data_ptr() or None), rows.numel()
                 if rows.numel() == 0 and skip_hubs:
                     return out
-        rc = lib().dgcn_genconv_aggregate_fused_rows(dtype, _ptr(x_src), _ptr(x_dst), N, C, _ptr(rowptr), _ptr(src),
+        rc = lib().dgcn_genconv_aggregate_fused_keep(dtype, _ptr(x_src), _ptr(x_dst), N, C, _ptr(rowptr), _ptr(src),
                                                      _ptr(eid), _ptr(edge_attr), ctypes.byref(prm),
                                                      ctypes.byref(hubs) if hubs is not None else None,
-                                                     ctypes.byref(fus) if fus is not None else None, _ptr(out),
+                                                     ctypes.byref(fus) if fus is not None else None,
+                                                     ctypes.byref(km) if km is not None else None, _ptr(out),
                                                      _stream(dev))
         _check(rc, "dgcn_genconv_aggregate")
     return out
 
 
 def genconv_aggregate_backward(x_src, x_dst, csr, prm, grad_out, edge_attr=None, softmax_grad=False,
-                               need_edge_attr=False):
-    """dgcn_genconv_aggregate_backward(_rows): (grad_x_src (N_src,C) fp32, grad_x_dst (N,C) fp32 | None,
-    grad_edge_attr in edge_attr's row dtype | None, grad_scalars (4) = d/dt, d/dp, d/dy, d/dmsg_scale)."""
+                               need_edge_attr=False, pre=None, keep=None):
+    """dgcn_genconv_aggregate_backward(_rows / _keep): (grad_x_src (N_src,C) fp32, grad_x_dst (N,C) fp32 | None,
+    grad_edge_attr in edge_attr's row dtype | None, grad_scalars (4) = d/dt, d/dp, d/dy, d/dmsg_scale).
+    pre / keep: the forward's (genconv_aggregate); the row gradients are then w.r.t. the activated rows."""
     rowptr, src, eid = csr[:3]
     _require_cuda(x_src, x_dst, grad_out, edge_attr)
-    dtype, x_src, x_dst, edge_attr = aggregate_rows(x_src, x_dst, edge_attr, backward=True)
+    dtype, x_src, x_dst, edge_attr = aggregate_rows(x_src, x_dst, edge_attr, pre=pre, backward=True)
+    km, _bits = _keep_mask(keep)
+    ps = ph = None
+    if pre is not None:
+        ps, ph = _f32(pre[0]), _f32(pre[1])
     grad_out = _f32(grad_out)
     N, C = rowptr.numel() - 1, x_src.shape[1]
     dev = x_src.device
@@ -629,12 +668,51 @@ def genconv_aggregate_backward(x_src, x_dst, csr, prm, grad_out, edge_attr=None,
             full = dtype != DTYPE_F32 and edge_attr.shape[0] == src.numel() and edge_attr.shape[0] > 1
             gea = torch.empty_like(edge_attr) if full else torch.zeros_like(edge_attr)
         gsc = torch.zeros(4, dtype=torch.float32, device=dev)
-        rc = lib().dgcn_genconv_aggregate_backward_rows(dtype, _ptr(x_src), _ptr(x_dst), N, x_src.shape[0], C,
+        rc = lib().dgcn_genconv_aggregate_backward_keep(dtype, _ptr(x_src), _ptr(x_dst), N, x_src.shape[0], C,
                                                         _ptr(rowptr), _ptr(src), _ptr(eid), _ptr(edge_attr),
-                                                        ctypes.byref(prm), int(bool(softmax_grad)), _ptr(grad_out),
+                                                        ctypes.byref(prm), int(bool(softmax_grad)), _ptr(ps), _ptr(ph),
+                                                        int(bool(pre[2])) if pre is not None else 0,
+                                                        ctypes.byref(km) if km is not None else None, _ptr(grad_out),
                                                         _ptr(gsrc), _ptr(gdst), _ptr(gea), _ptr(gsc), _stream(dev))
         _check(rc, "dgcn_genconv_aggregate_backward")
     return gsrc, gdst, gea, gsc
+
+
+def keep_bits(keep):
+    """dgcn_keep_bits_pack: keep (N, C) fp32 (non-zero = kept) -> (N, ceil(C / 32)) int32, bit c % 32 of word c / 32."""
+    _require_cuda(keep)
+    keep = _f32(keep)
+    N, C = keep.shape
+    with torch.cuda.device(keep.device):
+        bits = torch.empty((N, (C + 31) // 32), dtype=torch.int32, device=keep.device)
+        _check(lib().dgcn_keep_bits_pack(_ptr(keep), N, C, _ptr(bits), _stream(keep.device)), "dgcn_keep_bits_pack")
+    return bits
+
+
+def res_plus_backward_gy(h, scale, shift, keep, grad_src, grad_dst, mean=None, invstd=None):
+    """dgcn_res_plus_backward_gy: grad_src <- g_y (in place); returns the fp64 (2, C) [sum g_y | sum g_y * xhat]
+    when mean / invstd are given, else None."""
+    _require_cuda(h, grad_src, grad_dst)
+    N, C = h.shape
+    km, _bits = _keep_mask(keep)
+    with torch.cuda.device(h.device):
+        sums = torch.zeros((2, C), dtype=torch.float64, device=h.device) if mean is not None else None
+        _check(lib().dgcn_res_plus_backward_gy(_ptr(h), N, C, _ptr(scale), _ptr(shift),
+                                               ctypes.byref(km) if km is not None else None, _ptr(mean), _ptr(invstd),
+                                               _ptr(grad_src), _ptr(grad_dst), _ptr(sums), _stream(h.device)),
+               "dgcn_res_plus_backward_gy")
+    return sums
+
+
+def res_plus_backward_dh(g_y, h, a, b=None, d=None, grad_skip=None, out=None):
+    """dgcn_res_plus_backward_dh: a * g_y + b * h + d + grad_skip per channel (out may be grad_skip)."""
+    _require_cuda(g_y, h, grad_skip)
+    N, C = g_y.shape
+    with torch.cuda.device(g_y.device):
+        out = torch.empty_like(g_y) if out is None else out
+        _check(lib().dgcn_res_plus_backward_dh(_ptr(g_y), _ptr(h), N, C, _ptr(a), _ptr(b), _ptr(d), _ptr(grad_skip),
+                                               _ptr(out), _stream(g_y.device)), "dgcn_res_plus_backward_dh")
+    return out
 
 
 def linear_residual_supported(K, M):

@@ -63,6 +63,15 @@ struct KernelTimer {
   void* slot_;
 };
 
+// The res+ block's activated row in training, keep ? relu(s * x + t) * keep_scale : 0 (dgcn_keep_mask): one
+// function for the aggregate's reads and its backward's recomputation, so both see the same bits (__fmul_rn is
+// never contracted into an FMA).
+__device__ __forceinline__ float pre_keep(float s, float t, float x, bool relu, bool kept, float keep_scale) {
+  float z = fmaf(s, x, t);
+  if (relu) z = fmaxf(z, 0.f);
+  return kept ? __fmul_rn(z, keep_scale) : 0.f;
+}
+
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 

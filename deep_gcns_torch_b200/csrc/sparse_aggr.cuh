@@ -29,6 +29,8 @@ struct AggrArgs {
   // block fusion (dgcn_genconv_fusion): rows are read as act(pre_scale * x + pre_shift); MODE 0 walks row_list
   const float* pre_scale; const float* pre_shift; int pre_relu;
   const int32_t* row_list; int n_rows; int run_hubs;
+  // dropout folded into the pre-activation (dgcn_keep_mask; KEEP instantiations only)
+  const int32_t* keep_bits; int keep_words; float keep_scale;
 };
 
 
@@ -101,8 +103,12 @@ __device__ __forceinline__ int chan_of(int lane, int blk, int j) { return blk * 
 // T: element type of the rows (float, __nv_bfloat16, __half); the arithmetic is fp32 and identical for all three.
 // PRE: the block's norm -> relu is folded into the reads (dgcn_genconv_fusion); a separate instantiation so that
 // the plain kernel keeps its register budget (occupancy is what hides the gather latency).
-template <typename T, int VEC, int NBLK, int AGGR, int MODE, bool PRE>
-__global__ void __launch_bounds__(256, PRE ? 3 : 1) genconv_aggregate_kernel(const AggrArgs g) {
+// KEEP (with PRE, fp32 rows, no edge features): dropout too - each lane loads its VEC channels' keep bits from the
+// row's words next to the row itself and reads the row as pre_keep(...).
+// (two CTAs per SM for KEEP: the bits' registers would not fit the 85 of three without spilling at NBLK = 2, 4)
+template <typename T, int VEC, int NBLK, int AGGR, int MODE, bool PRE, bool KEEP = false>
+__global__ void __launch_bounds__(256, KEEP ? 2 : (PRE ? 3 : 1)) genconv_aggregate_kernel(const AggrArgs g) {
+  static_assert(!KEEP || (PRE && VEC == 4), "keep bits ride on the float4 pre-activation kernels");
   constexpr bool HUB = MODE == 1;
   __shared__ float hub_red[HUB ? 8 : 1][3][VEC][32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -158,6 +164,7 @@ __global__ void __launch_bounds__(256, PRE ? 3 : 1) genconv_aggregate_kernel(con
         for (int u0 = 0; u0 < cnt; u0 += 4) {
           VecF<VEC> xv[4], ev[4];
           bool have[4];
+          unsigned kb[4];   // KEEP: the lane's VEC keep bits of each edge's source row
 #pragma unroll
           for (int u = 0; u < 4; ++u) {
             const int s = __shfl_sync(0xffffffffu, my_src, (u0 + u) & 31);
@@ -169,8 +176,11 @@ __global__ void __launch_bounds__(256, PRE ? 3 : 1) genconv_aggregate_kernel(con
               xv[u].v[j] = 0.f;
               ev[u].v[j] = 0.f;
             }
+            if (KEEP) kb[u] = 0u;
             if (have[u]) {
               xv[u] = load_vec<VEC>(reinterpret_cast<const T*>(g.x_src) + static_cast<int64_t>(s) * C + cbase);
+              if (KEEP) kb[u] = static_cast<unsigned>(__ldg(g.keep_bits + static_cast<int64_t>(s) * g.keep_words +
+                                                            (cbase >> 5))) >> (cbase & 31);
               if (g.edge_attr) ev[u] = load_vec<VEC>(reinterpret_cast<const T*>(g.edge_attr) + static_cast<int64_t>(ei) * C + cbase);
             }
           }
@@ -180,7 +190,9 @@ __global__ void __launch_bounds__(256, PRE ? 3 : 1) genconv_aggregate_kernel(con
 #pragma unroll
             for (int u = 0; u < 4; ++u) {
               float v = xv[u].v[j];
-              if (pre) {   // applied here, behind all four row loads, so that the loads stay back to back
+              if (KEEP) {
+                v = pre_keep(ps[j], pt[j], v, g.pre_relu != 0, (kb[u] >> j) & 1u, g.keep_scale);
+              } else if (pre) {   // applied here, behind all four row loads, so that the loads stay back to back
                 v = fmaf(ps[j], v, pt[j]);
                 if (pre_relu_now) v = fmaxf(v, 0.f);
               }
@@ -325,7 +337,15 @@ __global__ void __launch_bounds__(256, PRE ? 3 : 1) genconv_aggregate_kernel(con
           ps[j] = __ldg(g.pre_scale + cbase + j);
           pt[j] = __ldg(g.pre_shift + cbase + j);
         }
-        pre_apply<VEC>(xv, ps, pt, true, g.pre_relu != 0);
+        if (KEEP) {
+          const unsigned kr = static_cast<unsigned>(__ldg(g.keep_bits + static_cast<int64_t>(row) * g.keep_words +
+                                                          (cbase >> 5))) >> (cbase & 31);
+#pragma unroll
+          for (int j = 0; j < VEC; ++j) xv.v[j] = pre_keep(ps[j], pt[j], xv.v[j], g.pre_relu != 0, (kr >> j) & 1u,
+                                                            g.keep_scale);
+        } else {
+          pre_apply<VEC>(xv, ps, pt, true, g.pre_relu != 0);
+        }
       }
 #pragma unroll
       for (int j = 0; j < VEC; ++j) xr[blk][j] = xv.v[j];
@@ -361,16 +381,16 @@ __global__ void __launch_bounds__(256, PRE ? 3 : 1) genconv_aggregate_kernel(con
   }   // hub_it
 }
 
-template <typename T, int VEC, int NBLK, bool PRE>
+template <typename T, int VEC, int NBLK, bool PRE, bool KEEP = false>
 static int launch_aggr(const AggrArgs& g, cudaStream_t stream) {
   const int warps = 8;
   const unsigned grid = static_cast<unsigned>(ceil_div(g.n_rows, warps));
 #define DGCN_AGGR_CASE(A)                                                                   \
   case A:                                                                                   \
-    if (grid) genconv_aggregate_kernel<T, VEC, NBLK, A, 0, PRE><<<grid, warps * 32, 0, stream>>>(g); \
+    if (grid) genconv_aggregate_kernel<T, VEC, NBLK, A, 0, PRE, KEEP><<<grid, warps * 32, 0, stream>>>(g); \
     if (g.hub_rows && g.run_hubs) {                                                                     \
-      genconv_aggregate_kernel<T, VEC, NBLK, A, 1, PRE><<<4 * device_sm_count(), 256, 0, stream>>>(g); \
-      genconv_aggregate_kernel<T, VEC, NBLK, A, 2, PRE><<<32, 256, 0, stream>>>(g);                 \
+      genconv_aggregate_kernel<T, VEC, NBLK, A, 1, PRE, KEEP><<<4 * device_sm_count(), 256, 0, stream>>>(g); \
+      genconv_aggregate_kernel<T, VEC, NBLK, A, 2, PRE, KEEP><<<32, 256, 0, stream>>>(g);                 \
     }                                                                                       \
     break;
   KernelTimer timer(stream, "aggregate");

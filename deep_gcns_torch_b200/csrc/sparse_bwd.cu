@@ -22,6 +22,10 @@ struct AggrBwdArgs {
   float eps; int msg_norm; float msg_scale; const float* msg_scale_dev; int add_residual; int raw;
   int softmax_grad;
   const float* gout; float* gx_src; float* gx_dst; float* gea; float* gscalars;
+  // PRE instantiations: rows are recomputed as the forward read them, pre_keep(pre_scale, pre_shift, x, pre_relu,
+  // keep bit, keep_scale); without keep bits every channel is kept and keep_scale is 1
+  const float* pre_scale; const float* pre_shift; int pre_relu;
+  const int32_t* keep_bits; int keep_words; float keep_scale;
 };
 
 // one row element, widened exactly to fp32 / rounded to nearest even from fp32 (what Tensor.to does)
@@ -33,8 +37,9 @@ template <> __device__ __forceinline__ float from_f32<float>(float v) { return v
 template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
 template <> __device__ __forceinline__ __half from_f32<__half>(float v) { return __float2half_rn(v); }
 
-// T: element type of the rows (float, __nv_bfloat16, __half); NCH: channels per lane (c = lane + 32*u)
-template <typename T, int NCH>
+// T: element type of the rows (float, __nv_bfloat16, __half); NCH: channels per lane (c = lane + 32*u, so channel
+// c's keep bit is bit `lane` of the row's word u); PRE: the forward's pre-activation (+ keep mask), fp32 rows.
+template <typename T, int NCH, bool PRE = false>
 __global__ void __launch_bounds__(256) genconv_aggregate_bwd_kernel(const AggrBwdArgs g) {
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -48,6 +53,20 @@ __global__ void __launch_bounds__(256) genconv_aggregate_bwd_kernel(const AggrBw
   const bool softmax = aggr == DGCN_AGGR_SOFTMAX || aggr == DGCN_AGGR_SOFTMAX_SUM;
   const bool power = aggr == DGCN_AGGR_POWER || aggr == DGCN_AGGR_POWER_SUM;
   const bool scaled = aggr == DGCN_AGGR_SOFTMAX_SUM || aggr == DGCN_AGGR_POWER_SUM;
+  float ps[NCH], pt[NCH];
+#pragma unroll
+  for (int u = 0; u < NCH; ++u) {
+    const int c = lane + 32 * u;
+    ps[u] = (PRE && c < C) ? __ldg(g.pre_scale + c) : 1.f;
+    pt[u] = (PRE && c < C) ? __ldg(g.pre_shift + c) : 0.f;
+  }
+  // the activated value of channel lane + 32*u of row r (identity without PRE)
+  auto act = [&](float x, int r, int u) {
+    if (!PRE) return x;
+    const bool kept = g.keep_bits == nullptr ||
+                      ((__ldg(g.keep_bits + static_cast<int64_t>(r) * g.keep_words + u) >> lane) & 1);
+    return pre_keep(ps[u], pt[u], x, g.pre_relu != 0, kept, g.keep_scale);
+  };
 
   // ---- pass A: recompute the aggregate ---------------------------------------------------------
   float M[NCH], S[NCH], W[NCH], L[NCH];   // running max, sum exp / count, weighted sum, sum u^p ln u
@@ -63,7 +82,7 @@ __global__ void __launch_bounds__(256) genconv_aggregate_bwd_kernel(const AggrBw
     for (int u = 0; u < NCH; ++u) {
       const int c = lane + 32 * u;
       if (c < C) {
-        float v = ld_row(reinterpret_cast<const T*>(g.x_src) + static_cast<int64_t>(s) * C + c);
+        float v = act(ld_row(reinterpret_cast<const T*>(g.x_src) + static_cast<int64_t>(s) * C + c), s, u);
         if (g.edge_attr) v += ld_row(reinterpret_cast<const T*>(g.edge_attr) + static_cast<int64_t>(ei) * C + c);
         const float msg = g.raw ? v : fmaxf(v, 0.f) + g.eps;
         if (softmax) {
@@ -113,7 +132,8 @@ __global__ void __launch_bounds__(256) genconv_aggregate_bwd_kernel(const AggrBw
   for (int u = 0; u < NCH; ++u) {
     const int c = lane + 32 * u;
     gh[u] = c < C ? __ldg(g.gout + static_cast<int64_t>(row) * C + c) : 0.f;
-    xr[u] = (need_x && c < C) ? ld_row(reinterpret_cast<const T*>(g.x_dst) + static_cast<int64_t>(row) * C + c) : 0.f;
+    xr[u] = (need_x && c < C) ? act(ld_row(reinterpret_cast<const T*>(g.x_dst) + static_cast<int64_t>(row) * C + c), row, u)
+                              : 0.f;
     n2m = fmaf(m[u], m[u], n2m);
     n2x = fmaf(xr[u], xr[u], n2x);
     dot_gm = fmaf(gh[u], m[u], dot_gm);
@@ -179,7 +199,7 @@ __global__ void __launch_bounds__(256) genconv_aggregate_bwd_kernel(const AggrBw
     for (int u = 0; u < NCH; ++u) {
       const int c = lane + 32 * u;
       if (c < C) {
-        float v = ld_row(reinterpret_cast<const T*>(g.x_src) + static_cast<int64_t>(s) * C + c);
+        float v = act(ld_row(reinterpret_cast<const T*>(g.x_src) + static_cast<int64_t>(s) * C + c), s, u);
         if (g.edge_attr) v += ld_row(reinterpret_cast<const T*>(g.edge_attr) + static_cast<int64_t>(ei) * C + c);
         const float msg = g.raw ? v : fmaxf(v, 0.f) + g.eps;
         float dmsg;
@@ -220,14 +240,14 @@ __global__ void __launch_bounds__(256) genconv_aggregate_bwd_kernel(const AggrBw
   }
 }
 
-template <typename T>
+template <typename T, bool PRE = false>
 static void launch_bwd(const AggrBwdArgs& g, cudaStream_t s) {
   const unsigned grid = static_cast<unsigned>(ceil_div(g.N, 8));
-  if (g.C <= 32) genconv_aggregate_bwd_kernel<T, 1><<<grid, 256, 0, s>>>(g);
-  else if (g.C <= 64) genconv_aggregate_bwd_kernel<T, 2><<<grid, 256, 0, s>>>(g);
-  else if (g.C <= 128) genconv_aggregate_bwd_kernel<T, 4><<<grid, 256, 0, s>>>(g);
-  else if (g.C <= 256) genconv_aggregate_bwd_kernel<T, 8><<<grid, 256, 0, s>>>(g);
-  else genconv_aggregate_bwd_kernel<T, 16><<<grid, 256, 0, s>>>(g);
+  if (g.C <= 32) genconv_aggregate_bwd_kernel<T, 1, PRE><<<grid, 256, 0, s>>>(g);
+  else if (g.C <= 64) genconv_aggregate_bwd_kernel<T, 2, PRE><<<grid, 256, 0, s>>>(g);
+  else if (g.C <= 128) genconv_aggregate_bwd_kernel<T, 4, PRE><<<grid, 256, 0, s>>>(g);
+  else if (g.C <= 256) genconv_aggregate_bwd_kernel<T, 8, PRE><<<grid, 256, 0, s>>>(g);
+  else genconv_aggregate_bwd_kernel<T, 16, PRE><<<grid, 256, 0, s>>>(g);
 }
 
 }  // namespace dgcn
@@ -251,12 +271,29 @@ extern "C" int dgcn_genconv_aggregate_backward_rows(int32_t dtype, const void* x
                                                     const dgcn_genconv_params* prm, int32_t softmax_grad,
                                                     const float* grad_out, float* grad_x_src, float* grad_x_dst,
                                                     void* grad_edge_attr, float* grad_scalars, dgcn_stream_t stream) {
+  return dgcn_genconv_aggregate_backward_keep(dtype, x_src, x_dst, N, N_src, C, rowptr, src, eid, edge_attr, prm,
+                                              softmax_grad, nullptr, nullptr, 0, nullptr, grad_out, grad_x_src,
+                                              grad_x_dst, grad_edge_attr, grad_scalars, stream);
+}
+
+extern "C" int dgcn_genconv_aggregate_backward_keep(int32_t dtype, const void* x_src, const void* x_dst, int64_t N,
+                                                    int64_t N_src, int64_t C, const int32_t* rowptr,
+                                                    const int32_t* src, const int32_t* eid, const void* edge_attr,
+                                                    const dgcn_genconv_params* prm, int32_t softmax_grad,
+                                                    const float* pre_scale, const float* pre_shift, int32_t pre_relu,
+                                                    const dgcn_keep_mask* keep, const float* grad_out,
+                                                    float* grad_x_src, float* grad_x_dst, void* grad_edge_attr,
+                                                    float* grad_scalars, dgcn_stream_t stream) {
   (void)N_src;
   if (!x_src || !rowptr || !src || !prm || !grad_out || N < 0 || C <= 0) return DGCN_ERR_BAD_ARG;
   if (dtype != DGCN_F32 && dtype != DGCN_BF16 && dtype != DGCN_F16) return DGCN_ERR_BAD_ARG;
   if (!x_dst && (prm->msg_norm || prm->add_residual)) return DGCN_ERR_BAD_ARG;
   if ((edge_attr || grad_edge_attr) && !eid) return DGCN_ERR_BAD_ARG;
   if (prm->aggr < DGCN_AGGR_SOFTMAX || prm->aggr > DGCN_AGGR_MAX) return DGCN_ERR_UNSUPPORTED;
+  if ((pre_scale == nullptr) != (pre_shift == nullptr)) return DGCN_ERR_BAD_ARG;
+  if (keep && (!keep->keep_bits || keep->words_per_row < (C + 31) / 32)) return DGCN_ERR_BAD_ARG;
+  if (pre_scale && dtype != DGCN_F32) return DGCN_ERR_UNSUPPORTED;
+  if (keep && (!pre_scale || !pre_relu || edge_attr || grad_edge_attr)) return DGCN_ERR_UNSUPPORTED;
   if (N == 0) return DGCN_OK;
   AggrBwdArgs g{};
   g.x_src = static_cast<const float*>(x_src); g.x_dst = static_cast<const float*>(x_dst);
@@ -267,9 +304,15 @@ extern "C" int dgcn_genconv_aggregate_backward_rows(int32_t dtype, const void* x
   g.eps = prm->eps; g.msg_norm = prm->msg_norm; g.msg_scale = prm->msg_scale; g.msg_scale_dev = prm->msg_scale_dev;
   g.add_residual = prm->add_residual; g.raw = prm->raw_message; g.softmax_grad = softmax_grad;
   g.gout = grad_out; g.gx_src = grad_x_src; g.gx_dst = grad_x_dst; g.gea = static_cast<float*>(grad_edge_attr); g.gscalars = grad_scalars;
+  g.pre_scale = pre_scale; g.pre_shift = pre_shift; g.pre_relu = pre_relu; g.keep_scale = 1.f;
+  if (keep) {
+    g.keep_bits = keep->keep_bits; g.keep_words = static_cast<int>(keep->words_per_row);
+    g.keep_scale = keep->keep_scale;
+  }
   if (C > 512 || (dtype != DGCN_F32 && (C % 4) != 0)) return DGCN_ERR_UNSUPPORTED;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (dtype == DGCN_BF16) launch_bwd<__nv_bfloat16>(g, s);
+  if (pre_scale) launch_bwd<float, true>(g, s);
+  else if (dtype == DGCN_BF16) launch_bwd<__nv_bfloat16>(g, s);
   else if (dtype == DGCN_F16) launch_bwd<__half>(g, s);
   else launch_bwd<float>(g, s);
   DGCN_LAUNCH_CHECK();

@@ -81,12 +81,24 @@ int dgcn_genconv_aggregate_fused_rows(int32_t dtype, const void* x_src, const vo
                                       const void* edge_attr, const dgcn_genconv_params* prm,
                                       const dgcn_csr_hubs* hubs, const dgcn_genconv_fusion* fus, float* out,
                                       dgcn_stream_t stream) {
+  return dgcn_genconv_aggregate_fused_keep(dtype, x_src, x_dst, N, C, rowptr, src, eid, edge_attr, prm, hubs, fus,
+                                           nullptr, out, stream);
+}
+
+int dgcn_genconv_aggregate_fused_keep(int32_t dtype, const void* x_src, const void* x_dst, int64_t N, int64_t C,
+                                      const int32_t* rowptr, const int32_t* src, const int32_t* eid,
+                                      const void* edge_attr, const dgcn_genconv_params* prm,
+                                      const dgcn_csr_hubs* hubs, const dgcn_genconv_fusion* fus,
+                                      const dgcn_keep_mask* keep, float* out, dgcn_stream_t stream) {
   if (!x_src || !rowptr || !src || !prm || !out || N < 0 || C <= 0) return DGCN_ERR_BAD_ARG;
   if (dtype != DGCN_F32 && dtype != DGCN_BF16 && dtype != DGCN_F16) return DGCN_ERR_BAD_ARG;
   if (fus && ((fus->pre_scale == nullptr) != (fus->pre_shift == nullptr))) return DGCN_ERR_BAD_ARG;
   if (fus && fus->row_list && (fus->n_rows < 0 || fus->n_rows > N)) return DGCN_ERR_BAD_ARG;
   if (!x_dst && (prm->msg_norm || prm->add_residual)) return DGCN_ERR_BAD_ARG;
   if (edge_attr && !eid) return DGCN_ERR_BAD_ARG;
+  if (keep && (!keep->keep_bits || keep->words_per_row < (C + 31) / 32)) return DGCN_ERR_BAD_ARG;
+  if (keep && (dtype != DGCN_F32 || !fus || !fus->pre_scale || !fus->pre_relu || edge_attr))
+    return DGCN_ERR_UNSUPPORTED;
   if (N == 0) return DGCN_OK;
   if (N > (1ll << 31) - 1) return DGCN_ERR_UNSUPPORTED;
   AggrArgs g{};
@@ -106,6 +118,10 @@ int dgcn_genconv_aggregate_fused_rows(int32_t dtype, const void* x_src, const vo
     if (fus->row_list) { g.row_list = fus->row_list; g.n_rows = static_cast<int>(fus->n_rows); }
     g.run_hubs = fus->skip_hubs ? 0 : 1;
   }
+  if (keep) {
+    g.keep_bits = keep->keep_bits; g.keep_words = static_cast<int>(keep->words_per_row);
+    g.keep_scale = keep->keep_scale;
+  }
   if (hubs && hubs->rows && hubs->items && hubs->counts && hubs->partial && hubs->min_degree > 0 &&
       hubs->seg_edges > 0) {
     g.hub_items = hubs->items; g.hub_item_count = hubs->counts; g.hub_rows = hubs->rows;
@@ -123,6 +139,12 @@ int dgcn_genconv_aggregate_fused_rows(int32_t dtype, const void* x_src, const vo
   const bool aligned = ((reinterpret_cast<uintptr_t>(x_src) | reinterpret_cast<uintptr_t>(x_dst) |
                          reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(edge_attr)) & 15) == 0;
   if ((C % 4) == 0 && aligned) {
+    if (g.keep_bits) {   // pre-activation + dropout (the res+ block in training)
+      if (C <= 128) return launch_aggr<float, 4, 1, true, true>(g, s);
+      if (C <= 256) return launch_aggr<float, 4, 2, true, true>(g, s);
+      if (C <= 512) return launch_aggr<float, 4, 4, true, true>(g, s);
+      return DGCN_ERR_UNSUPPORTED;
+    }
     if (g.pre_scale) {   // fused pre-activation: float4 channel blocks only
       if (C <= 128) return launch_aggr<float, 4, 1, true>(g, s);
       if (C <= 256) return launch_aggr<float, 4, 2, true>(g, s);

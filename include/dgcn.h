@@ -333,6 +333,31 @@ int dgcn_genconv_aggregate_fused_rows(int32_t dtype, const void* x_src, const vo
                                       const dgcn_genconv_fusion* fus /* may be NULL */, float* out,
                                       dgcn_stream_t stream);
 
+/* Dropout folded into the pre-activation of the res+ block in training (examples/ogb/ogbn_arxiv/model.py:91-106:
+ * dropout(relu(norm(h)))).  keep_bits (N_src, words_per_row) int32 words, bit c % 32 of word c / 32 set when
+ * channel c of that row is kept; words_per_row >= ceil(C / 32).  Row r of x_src and row r of x_dst (the first N
+ * rows of x_src's numbering) use bit row r.  With it every row read from x_src and x_dst is taken as
+ *   keep ? relu(pre_scale * x + pre_shift) * keep_scale : 0          (keep_scale = 1 / (1 - p)),
+ * computed in this order in fp32 by the forward and the backward, so both see the same values. */
+typedef struct dgcn_keep_mask {
+  const int32_t* keep_bits;
+  int64_t words_per_row;
+  float keep_scale;
+} dgcn_keep_mask;
+/* dgcn_genconv_aggregate_fused_rows plus a keep mask (NULL: exactly dgcn_genconv_aggregate_fused_rows).  A keep
+ * mask needs fp32 rows, a pre-activation with pre_relu != 0 and no edge_attr; anything else returns
+ * DGCN_ERR_UNSUPPORTED. */
+int dgcn_genconv_aggregate_fused_keep(int32_t dtype, const void* x_src, const void* x_dst, int64_t N, int64_t C,
+                                      const int32_t* rowptr, const int32_t* src, const int32_t* eid,
+                                      const void* edge_attr, const dgcn_genconv_params* prm,
+                                      const dgcn_csr_hubs* hubs /* may be NULL */,
+                                      const dgcn_genconv_fusion* fus /* may be NULL */,
+                                      const dgcn_keep_mask* keep /* may be NULL */, float* out,
+                                      dgcn_stream_t stream);
+/* Bit-pack a keep mask: keep (N, C) fp32 (non-zero = kept, what Tensor.bernoulli_ draws) -> keep_bits
+ * (N, ceil(C / 32)) int32 in the dgcn_keep_mask layout (bits of channels >= C are 0). */
+int dgcn_keep_bits_pack(const float* keep, int64_t N, int64_t C, int32_t* keep_bits, dgcn_stream_t stream);
+
 /* Row-wise Linear with fused bias and skip connection on the tensor cores (wgmma):
  *   out[n][m] = sum_k a[n][k] * weight[m][k] (+ bias[m]) (+ res[n][m])
  * = the Linear that ends GENConv's MLP (gcn_lib/sparse/torch_nn.py:56-68 with mlp_layers = 1; nn.Linear
@@ -372,6 +397,33 @@ int dgcn_genconv_aggregate_backward_rows(int32_t dtype, const void* x_src, const
                                          int32_t softmax_grad, const float* grad_out,
                                          float* grad_x_src, float* grad_x_dst, void* grad_edge_attr,
                                          float* grad_scalars, dgcn_stream_t stream);
+/* The same with the forward's pre-activation (pre_scale / pre_shift (C) or both NULL, pre_relu; see
+ * dgcn_genconv_fusion) and keep mask (dgcn_keep_mask, may be NULL): the rows are recomputed from x exactly as the
+ * forward read them, and grad_x_src / grad_x_dst are the gradients w.r.t. those activated rows (the caller applies
+ * the chain rule through the pre-activation).  Without both it is dgcn_genconv_aggregate_backward_rows.  A
+ * pre-activation needs fp32 rows; a keep mask needs a pre-activation with pre_relu != 0 and no edge_attr; C > 512
+ * is unsupported; anything else returns DGCN_ERR_UNSUPPORTED. */
+int dgcn_genconv_aggregate_backward_keep(int32_t dtype, const void* x_src, const void* x_dst, int64_t N,
+                                         int64_t N_src, int64_t C, const int32_t* rowptr,
+                                         const int32_t* src, const int32_t* eid,
+                                         const void* edge_attr, const dgcn_genconv_params* prm,
+                                         int32_t softmax_grad, const float* pre_scale, const float* pre_shift,
+                                         int32_t pre_relu, const dgcn_keep_mask* keep /* may be NULL */,
+                                         const float* grad_out, float* grad_x_src, float* grad_x_dst,
+                                         void* grad_edge_attr, float* grad_scalars, dgcn_stream_t stream);
+/* Backward epilogue of the fused res+ block in training: one pass over (N, C) rows
+ *   g_y = (g_src + g_dst) * (keep ? keep_scale : 0) * [pre_scale * h + pre_shift > 0]      written over g_src,
+ * the gradient w.r.t. the BatchNorm output (keep may be NULL: all kept, scale 1), and per channel
+ *   sums[c] += sum_rows g_y,   sums[C + c] += sum_rows g_y * (h - mean[c]) * invstd[c]
+ * (fp64, zero-initialised by the caller; the BatchNorm's d beta and d gamma / gamma). */
+int dgcn_res_plus_backward_gy(const float* h, int64_t N, int64_t C, const float* pre_scale, const float* pre_shift,
+                              const dgcn_keep_mask* keep /* may be NULL */, const float* mean, const float* invstd,
+                              float* grad_src, const float* grad_dst, double* sums, dgcn_stream_t stream);
+/* ... and its second pass: grad_h = a[c] * g_y + b[c] * h + d[c] + grad_skip (grad_h may alias g_y or grad_skip), the
+ * BatchNorm backward folded per channel by the caller (batch statistics: a = gamma * invstd,
+ * b = -a * invstd * mean(g_y * xhat), d = -a * mean(g_y) - b * mean; running statistics: a = scale, b = d = 0). */
+int dgcn_res_plus_backward_dh(const float* g_y, const float* h, int64_t N, int64_t C, const float* a, const float* b,
+                              const float* d, const float* grad_skip, float* grad_h, dgcn_stream_t stream);
 
 /* Halo packing for node-partitioned graphs (new functionality; the reference
  * has no multi-GPU sparse path, SURVEY.md 3.4): out[r,:] = x[rows[r],:]. */

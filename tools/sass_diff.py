@@ -33,6 +33,11 @@ def kernels(obj):
 
 def normalise(name):
     name = re.sub(r"^void ", "", name)
+    # the trailing template flag the GENConv kernels gained last (KEEP of the aggregate: 7th argument, PRE of its
+    # backward: 3rd) is false for every kernel that existed before it
+    m = re.match(r"^(?:dgcn::)?genconv_aggregate(_bwd)?_kernel<([^>]*)>", name)
+    if m and m.group(2).endswith(", (bool)0") and len(m.group(2).split(",")) == (3 if m.group(1) else 7):
+        name = name.replace(m.group(2), m.group(2)[:-len(", (bool)0")], 1)
     name = name.replace("<float, ", "<")
     return re.sub(r"<float>\(const T1 \*, (.*), T1 \*\)", r"(const float *, \1, float *)", name)
 

@@ -371,6 +371,8 @@ struct TcArgs {
   CUtensorMap tm_planes;         // bf16 (B*2*Cpad rows, N) - fp16 (B*Cpad rows, N) for knn_tc4_kernel - row-major,
                                  // box 64 points x Cpad rows, SWIZZLE_128B
   CUtensorMap tm_sqp;            // bf16 (B*8 rows, N), box 64 points x 8 rows, SWIZZLE_128B
+  CUtensorMap tm_cand;           // knn_tc4_kernel's candidate tiles: the fp16 plane, box 32 points x Cpad rows, SWIZZLE_64B
+  CUtensorMap tm_sqc;            // knn_tc4_kernel: sqp, box 32 points x 8 rows, SWIZZLE_64B
   KnnArgs a;
   const __nv_bfloat16* planes;   // (B,2,Cpad,N) bf16, or (B,1,Cpad,N) fp16 for knn_tc4_kernel
   const __nv_bfloat16* sqp;      // (B,8,N): rows 0..2 = bf16 split of -|x|^2/2, rest zero

@@ -2,30 +2,39 @@
 //
 //   Why: the CTA holds T4_GROUPS query tiles of the SAME cloud, so a candidate tile is brought in once (TMA) and
 //   multiplied against every resident query operand, and the filter code of knn_tc_kernel is replaced by a cheaper
-//   sorting-network flush.  Two groups: the query planes, the per-group accumulator stage and candidate buffer of a
-//   third would not fit the 227 KB of shared memory an H100 block may use.
+//   sorting-network flush.  Four groups: the filter's serial chains (slot-pointer bump, the vote every 8 candidates,
+//   LDS latency, the barriers) are hidden by four filter warps per scheduler better than by two, and each group
+//   starts tile h + 1's wgmma before it filters tile h, so its own tensor work leaves its critical path (DESIGN.md
+//   4a).  Four fit the 227 KB of shared memory an H100 block may use because a candidate tile is 32 points
+//   wide, which halves the accumulator stage (18 KB per group), and because the epilogue's work area reuses the
+//   group's query plane, dead once its last wgmma has completed.  No separate producer warp: a 17th warp would put five warps on one scheduler and cap a
+//   thread at 96 registers; at 512 threads the cap is 128, which the kernel meets without spills, and thread 0
+//   issues the TMA between its own wgmma (produce below).
 //
 //   Operands: ONE fp16 plane (tc_prologue with f16), not knn_tc_kernel's bf16 (hi, mid) split.  The list entries keep
 //   20 bits of the distance, a resolution delta(v) = 2^-10 (v + |x_i|^2) (~0.14 at rank 20 of a 64-d normal cloud);
 //   the three-product bf16 split (~2^-14 relative, eps ~0.012 there) decided membership ~10x finer than the list can
 //   hold it; a single fp16 product (11-bit significand; with the per-query bound below, eps ~0.08) is of the same
-//   order as delta.  That is 10 instead of 26 m64n64k16 wgmma per half-tile and group at Cpad = 64, and half the
+//   order as delta.  That is 10 instead of 26 wgmma per 64 candidates and group at Cpad = 64, and half the
 //   operand bytes (TMA, shared memory, the wgmma's reads); the price is a list of 32 instead of 28 entries and a band of up to 16 instead of 12 (DESIGN.md 6).
 //
-//   producer warp            moves the operands by TMA: the query planes of the groups once, then 64-candidate
-//                            half-tiles into a two-stage ring (the stage of half-tile h+1 is refilled as soon as every
-//                            group has finished its wgmma on half-tile h-1, stage_free).
-//   filter warpgroup g       per half-tile: wait full[s], two m64n64k16 wgmma chains (query rows 0..63 and 64..127,
-//                            Cpad/16 fp16 + 1 bf16 each) against the stage, release the stage, the accumulators to the
-//                            group's shared-memory stage (row = query); thread r = query r of tile g reads 8 columns at a
-//                            time, threshold test -> private candidate buffer (shared memory, slot-major).
+//   thread 0 (group 0)       moves the operands by TMA: the query planes of the groups once (64-point boxes,
+//                            SWIZZLE_128B), then 32-candidate tiles (32-point boxes, SWIZZLE_64B) into a four-stage
+//                            ring (the stage of tile h is refilled once every group has finished its wgmma on
+//                            tile h - 4, stage_free; checked without blocking until group 0 needs tile h itself).
+//   filter warpgroup g       per tile h: wait for tile h's wgmma (started one tile earlier), release its stage, the
+//                            accumulators to the group's shared-memory stage (row = query); start tile h + 1's two
+//                            m64n32k16 wgmma chains (query rows 0..63 and 64..127, Cpad/16 fp16 + 1 bf16 each); then
+//                            thread r = query r of tile g reads tile h's 8 columns at a time, threshold test ->
+//                            private candidate buffer (shared memory, slot-major).
 //                            FLUSH = sorting network instead of one insertion per entry: the batch (<= 16 entries
 //                            per lane, a second pass for slots 16..23) is bitonic-sorted in registers, min-merged
 //                            against the upper half of the 32-entry sorted register list and the list re-sorted by
 //                            one 32-input bitonic merge - a fixed ~450 instructions per warp-wide flush whatever
 //                            the lanes' counts (the insertion loop costs ~80 per ROUND, rounds = the fullest
 //                            lane's count).
-//                            Then, per warpgroup (named barriers) in the group's own (now idle) accumulator stage:
+//                            Then, per warpgroup (named barriers) in the group's own (now idle) query plane and
+//                            accumulator stage, 34 KB contiguous:
 //                            - set-only consumers (every rank kept, no index output, no self exclusion): membership
 //                              by interval arithmetic on the approximate list, exact fp32 chains only inside the
 //                              ambiguous band around rank K (DESIGN.md 6);
@@ -40,36 +49,39 @@
 
 namespace dgcn {
 
-constexpr int T4_GROUPS = 2;
-constexpr int T4_THREADS = T4_GROUPS * 128 + 32;                 // filter warpgroups + the producer warp
-constexpr int T4_CT = 64;                                        // candidates per half-tile (wgmma N)
-constexpr int T4_STAGES = 2;
+constexpr int T4_GROUPS = 4;
+constexpr int T4_THREADS = T4_GROUPS * 128;                      // filter warpgroups; thread 0 also issues the TMA
+constexpr int T4_CT = 32;                                        // candidates per tile (wgmma N)
+constexpr int T4_STAGES = 4;
 constexpr int T4_CAP = 24;                                       // candidate-buffer slots per thread
 constexpr int T4_FLUSH_AT = 16;                                  // flush when a lane holds this many (checked every 8 candidates)
 constexpr int T4_LIST = 32;                                      // register list length (power of two >= KP)
 constexpr int T4_QBYTES = 2 * TC_MAX_C * 128;                    // 16 KB: fp16 query plane of one group (2 MN blocks)
-constexpr int T4_STAGE_BYTES = TC_MAX_C * 128;                   // 8 KB: one 64-candidate fp16 half-tile
+constexpr int T4_STAGE_BYTES = TC_MAX_C * 64;                    // 4 KB: one 32-candidate fp16 tile (64-byte rows)
 constexpr int T4_MB = 16;                                        // band entries a query may hold (set-only path)
-constexpr int T4_SX_BYTES = 16 * 128;                            // 2 KB: candidate-side extra K=16 block
+constexpr int T4_SX_BYTES = 16 * 64;                             // 1 KB: candidate-side extra K=16 block
 constexpr int T4_CBUF_BYTES = T4_CAP * 128 * 4;                  // 12 KB per group
-constexpr int T4_ACC_LD = 68;                                    // accumulator stage row: 64 columns + 4
-constexpr int T4_ACC_BYTES = TILE * T4_ACC_LD * 4;               // 34 KB per group
+constexpr int T4_ACC_LD = 36;                                    // accumulator stage row: 32 columns + 4
+constexpr int T4_ACC_BYTES = TILE * T4_ACC_LD * 4;               // 18 KB per group
+constexpr int T4_GROUP_BYTES = T4_QBYTES + T4_ACC_BYTES;         // 34 KB: [query plane | accumulator stage] of a group
 constexpr uint32_t T4_SLOT_STRIDE = 128u * 4u;                   // bytes between two slots of one thread
 static_assert(T4_SLOT_STRIDE == 512u, "the filter's asm bumps the slot pointer by the literal 512");
+static_assert(T4_GROUP_BYTES % 1024 == 0 && T4_STAGE_BYTES % 1024 == 0, "SWIZZLE_128B / 64B atoms stay aligned");
+static_assert((T4_STAGES & (T4_STAGES - 1)) == 0, "ring index by mask");
 
 struct T4Tail {
-  uint64_t full[T4_STAGES];               // half-tile operands have landed (TMA complete_tx)
+  uint64_t full[T4_STAGES];               // tile operands have landed (TMA complete_tx)
   uint64_t stage_free[T4_STAGES];         // every wgmma reading the stage has completed
   uint64_t q_full;                        // query planes have landed
   unsigned char ok[T4_GROUPS][TILE];
 };
 
-constexpr size_t T4_SMEM_BYTES = static_cast<size_t>(T4_GROUPS) * T4_QBYTES + T4_STAGES * (T4_STAGE_BYTES + T4_SX_BYTES) +
-                                 TC_XBLOCK_BYTES + static_cast<size_t>(T4_GROUPS) * (T4_CBUF_BYTES + T4_ACC_BYTES) +
-                                 sizeof(T4Tail) + 1024;
+constexpr size_t T4_SMEM_BYTES = static_cast<size_t>(T4_GROUPS) * T4_GROUP_BYTES + T4_STAGES * (T4_STAGE_BYTES + T4_SX_BYTES) +
+                                 TC_XBLOCK_BYTES + static_cast<size_t>(T4_GROUPS) * T4_CBUF_BYTES + sizeof(T4Tail) + 1024;
 static_assert(T4_SMEM_BYTES <= 227 * 1024, "one CTA per SM");
-// after the loop a group's accumulator stage holds the band (exact keys + indices) or the exact-sorted list
-static_assert(T4_MB * TILE * (8 + 4) <= T4_ACC_BYTES && T4_LIST * TILE * 8 <= T4_ACC_BYTES, "work areas");
+// after the loop a group's query plane and accumulator stage hold the band (exact keys + indices) or the
+// exact-sorted list
+static_assert(T4_MB * TILE * (8 + 4) <= T4_GROUP_BYTES && T4_LIST * TILE * 8 <= T4_GROUP_BYTES, "work areas");
 
 // compare-exchange of two register entries (ascending)
 __device__ __forceinline__ void t4_ce(uint32_t& x, uint32_t& y) {
@@ -107,18 +119,6 @@ __device__ __forceinline__ void t4_merge(uint32_t (&v)[NN]) {
     }
   }
 }
-// true on exactly one lane of the (converged) warp
-__device__ __forceinline__ bool t4_elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n"
-      ".reg .pred P;\n"
-      "elect.sync _|P, 0xffffffff;\n"
-      "selp.u32 %0, 1, 0, P;\n"
-      "}"
-      : "=r"(pred));
-  return pred != 0;
-}
 __device__ __forceinline__ void t4_group_sync(int g) {
   asm volatile("bar.sync %0, %1;" ::"r"(g + 1), "n"(128) : "memory");
 }
@@ -128,13 +128,13 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
   static_assert(KP <= T4_LIST && (KP & 1) == 0, "list length");
   extern __shared__ __align__(16) unsigned char smem_raw[];
   unsigned char* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // SWIZZLE_128B atoms: 1024-aligned
-  unsigned char* qbase = base;                                              // [group][mn block][Cpad rows][128 B]
-  unsigned char* stage0 = qbase + T4_GROUPS * T4_QBYTES;                    // [stage][Cpad rows][128 B]
-  unsigned char* sx0 = stage0 + T4_STAGES * T4_STAGE_BYTES;                 // [stage][16 rows][128 B]
+  // [group][query plane: mn block][Cpad rows][128 B] | accumulator stage: [128 queries][T4_ACC_LD] fp32]
+  unsigned char* gbase = base;
+  unsigned char* stage0 = gbase + T4_GROUPS * T4_GROUP_BYTES;               // [stage][Cpad rows][64 B]
+  unsigned char* sx0 = stage0 + T4_STAGES * T4_STAGE_BYTES;                 // [stage][16 rows][64 B]
   unsigned char* qx = sx0 + T4_STAGES * T4_SX_BYTES;                        // ones block, shared by the groups
   unsigned char* cbuf0 = qx + TC_XBLOCK_BYTES;                              // [group][slot][128 threads] u32
-  float* acc0 = reinterpret_cast<float*>(cbuf0 + T4_GROUPS * T4_CBUF_BYTES); // [group][128 queries][T4_ACC_LD]
-  T4Tail& sm = *reinterpret_cast<T4Tail*>(reinterpret_cast<unsigned char*>(acc0) + T4_GROUPS * T4_ACC_BYTES);
+  T4Tail& sm = *reinterpret_cast<T4Tail*>(cbuf0 + T4_GROUPS * T4_CBUF_BYTES);
   const KnnArgs& a = t.a;
   const int tid = threadIdx.x, warp = tid >> 5;
   const int b = blockIdx.y;
@@ -142,11 +142,12 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
   const int qt0 = blockIdx.x * T4_GROUPS;                                   // first query tile of this CTA
   const int ngroups = min(T4_GROUPS, N / TILE - qt0);
   const int H = N / T4_CT;
-  const int plane_q = 2 * Cpad * 128, plane_c = Cpad * 128;               // fp16 query plane / candidate half-tile
+  const int plane_q = 2 * Cpad * 128, plane_c = Cpad * 64;                // fp16 query plane / candidate tile
 
   if (tid == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&t.tm_planes)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&t.tm_sqp)) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&t.tm_cand)) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&t.tm_sqc)) : "memory");
     for (int s = 0; s < T4_STAGES; ++s) {
       mbar_init(&sm.full[s], 1);
       mbar_init(&sm.stage_free[s], static_cast<uint32_t>(ngroups * 128));
@@ -155,7 +156,7 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   // constant operand blocks: ones in K rows 0..2 on the query side; the candidate-side blocks are zero in rows
-  // 8..15 (TMA refreshes rows 0..7 of a stage with every half-tile).  Whole rows are constant: no swizzle needed.
+  // 8..15 (TMA refreshes rows 0..7 of a stage with every tile).  Whole rows are constant: no swizzle needed.
   for (int ch = tid; ch < TC_XBLOCK_BYTES / 16; ch += T4_THREADS) {
     const int row = (ch >> 3) & 15;
     const uint32_t one2 = row < 3 ? 0x3F803F80u : 0u;
@@ -166,36 +167,44 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
   fence_proxy_async();
   __syncthreads();
 
-  if (warp >= T4_GROUPS * 4) {
-    // ================================ producer: TMA ================================
-    const uint32_t tile_bytes = static_cast<uint32_t>(plane_c + 8 * 128);
-    auto tma_tile = [&](int h) {
-      const int s = h & 1;
-      mbar_expect_tx(&sm.full[s], tile_bytes);
-      tma_load_2d(smem_u32(stage0 + s * T4_STAGE_BYTES), &t.tm_planes, h * T4_CT, b * Cpad, &sm.full[s]);
-      tma_load_2d(smem_u32(sx0 + s * T4_SX_BYTES), &t.tm_sqp, h * T4_CT, b * 8, &sm.full[s]);
-    };
-    if (t4_elect_one()) {
-      mbar_expect_tx(&sm.q_full, static_cast<uint32_t>(ngroups * plane_q));
-      for (int g = 0; g < ngroups; ++g)
-#pragma unroll
-        for (int blk = 0; blk < 2; ++blk)
-          tma_load_2d(smem_u32(qbase + g * T4_QBYTES) + blk * (Cpad * 128), &t.tm_planes, (qt0 + g) * TILE + blk * 64,
-                      b * Cpad, &sm.q_full);
-      tma_tile(0);
-#pragma unroll 1
-      for (int h = 0; h + 1 < H; ++h) {                    // refill the other stage: its wgmma (half-tile h-1) must be done
-        if (h >= 1) mbar_wait_hint(&sm.stage_free[(h + 1) & 1], static_cast<uint32_t>(((h - 1) >> 1) & 1), 1000u);
-        tma_tile(h + 1);
-      }
-    }
-    __syncwarp();
-  } else {
-    if ((warp >> 2) < ngroups) {
+  if ((warp >> 2) < ngroups) {
     // ================================ filter warpgroup ================================
     const int g = warp >> 2;
     const int r = tid & 127;                               // query row of the tile
     const int q0 = (qt0 + g) * TILE, qg = q0 + r;
+
+    // TMA, issued by thread 0 (group 0 always exists): the query planes once, then the ring.  Tile `next` goes into
+    // its stage once every group has finished its wgmma on tile next - T4_STAGES (stage_free).  produce(need) waits
+    // for the stages of the tiles below `need` and then issues, without waiting, every further tile whose stage is
+    // already free - the group-0 thread never stalls on a slower group before it needs the tile itself.
+    const bool producer = tid == 0;
+    int next = 0;                                          // first tile not yet issued (producer thread)
+    auto produce = [&](int need) {
+      const uint32_t tile_bytes = static_cast<uint32_t>(plane_c + 8 * 64);
+#pragma unroll 1
+      while (next < H) {
+        const int s = next & (T4_STAGES - 1);
+        if (next >= T4_STAGES) {
+          const uint32_t par = static_cast<uint32_t>((next / T4_STAGES - 1) & 1);
+          if (next < need) mbar_wait_hint(&sm.stage_free[s], par, 1000u);
+          else if (!mbar_test(&sm.stage_free[s], par)) break;
+        }
+        mbar_expect_tx(&sm.full[s], tile_bytes);
+        tma_load_2d(smem_u32(stage0 + s * T4_STAGE_BYTES), &t.tm_cand, next * T4_CT, b * Cpad, &sm.full[s]);
+        tma_load_2d(smem_u32(sx0 + s * T4_SX_BYTES), &t.tm_sqc, next * T4_CT, b * 8, &sm.full[s]);
+        ++next;
+      }
+    };
+    if (producer) {
+      mbar_expect_tx(&sm.q_full, static_cast<uint32_t>(ngroups * plane_q));
+      for (int gq = 0; gq < ngroups; ++gq)
+#pragma unroll
+        for (int blk = 0; blk < 2; ++blk)
+          tma_load_2d(smem_u32(gbase + gq * T4_GROUP_BYTES) + blk * (Cpad * 128), &t.tm_planes,
+                      (qt0 + gq) * TILE + blk * 64, b * Cpad, &sm.q_full);
+      produce(0);
+    }
+    __syncwarp();
     const float* sqb = a.sq + static_cast<int64_t>(b) * N;
     uint32_t lk[T4_LIST];                                  // ascending packed entries (key bits | 12-bit index)
 #pragma unroll
@@ -278,43 +287,57 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
           "f"(__uint_as_float(V[6])), "f"(__uint_as_float(V[7])), "r"(RB), "f"(thr_acc));                             \
     if (__any_sync(0xffffffffu, cb_addr - cb_addr0 >= T4_FLUSH_AT * T4_SLOT_STRIDE)) flush();                         \
   } while (0)
-    // A half-tile is consumed in eight steps of 8 columns, two steps per iteration of a rolled loop (the flush code
+    // A tile is consumed in four steps of 8 columns, two steps per iteration of a rolled loop (the flush code
     // exists twice plus the final flush, not once per step: the instruction cache matters at ~700 instructions a copy).
-    const uint32_t abase = smem_u32(qbase + g * T4_QBYTES);
+    unsigned char* gb = gbase + g * T4_GROUP_BYTES;
+    const uint32_t abase = smem_u32(gb);
     const uint64_t dqx0 = wg_desc_sw128(smem_u32(qx), 2048, 1024), dqx1 = wg_desc_sw128(smem_u32(qx) + 2048, 2048, 1024);
-    float* accg = acc0 + g * (TILE * T4_ACC_LD);
+    float* accg = reinterpret_cast<float*>(gb + T4_QBYTES);
     const float* arow = accg + r * T4_ACC_LD;
+    // Tile j's wgmma: wait for its operands, start the two chains, do not wait for them.  Query rows 0..63 and
+    // 64..127 against the 32 staged candidates: one fp16 product x_i.x_j, then (bf16, into the same fp32 accumulators)
+    // + 1 x (-|x_j|^2/2).  The candidate side is one 32-wide SWIZZLE_64B block: 16 K rows of 64 B per wgmma, 512 B
+    // per 8 K rows.
+    float d0[16], d1[16];
+    auto mma = [&](int j) {
+      const int s = j & (T4_STAGES - 1);
+      if (producer) produce(j + 1);
+      __syncwarp();
+      mbar_wait_hint(&sm.full[s], static_cast<uint32_t>((j / T4_STAGES) & 1), 1000u);
+      const uint32_t bbase = smem_u32(stage0 + s * T4_STAGE_BYTES);
+      wg_fence();
+#pragma unroll 1
+      for (int kk = 0; kk < Cpad / 16; ++kk) {
+        const uint32_t ah = abase + kk * 2048;
+        const uint64_t db = wg_desc_sw64(bbase + kk * 1024, Cpad * 64, 512);
+        const uint32_t acc = kk > 0 ? 1u : 0u;
+        wgmma_m64n32<1, 1, WG_F16>(d0, wg_desc_sw128(ah, Cpad * 128, 1024), db, acc);
+        wgmma_m64n32<1, 1, WG_F16>(d1, wg_desc_sw128(ah + Cpad * 128, Cpad * 128, 1024), db, acc);
+      }
+      const uint64_t dsx = wg_desc_sw64(smem_u32(sx0 + s * T4_SX_BYTES), 1024, 512);
+      wgmma_m64n32<1, 1, WG_BF16>(d0, dqx0, dsx, 1u);
+      wgmma_m64n32<1, 1, WG_BF16>(d1, dqx1, dsx, 1u);
+      wg_commit();
+    };
+    // Software pipeline: tile h + 1's wgmma runs while the group filters tile h, so a group's own tensor work is not
+    // on its critical path (the accumulators of h + 1 stay in registers, the filter reads tile h from the stage).
     mbar_wait(&sm.q_full, 0u);
+    mma(0);
 #pragma unroll 1
     for (int h = 0; h < H; ++h) {
-      const int s = h & 1;
-      mbar_wait_hint(&sm.full[s], static_cast<uint32_t>((h >> 1) & 1), 1000u);
       {
-        // query rows 0..63 and 64..127 against the 64 staged candidates: one fp16 product x_i.x_j, then (bf16,
-        // into the same fp32 accumulators) + 1 x (-|x_j|^2/2)
-        const uint32_t bbase = smem_u32(stage0 + s * T4_STAGE_BYTES);
-        float d0[32], d1[32];
-        wg_fence();
-#pragma unroll 1
-        for (int kk = 0; kk < Cpad / 16; ++kk) {
-          const uint32_t ah = abase + kk * 2048;
-          const uint64_t db = wg_desc_sw128(bbase + kk * 2048, Cpad * 128, 1024);
-          const uint32_t acc = kk > 0 ? 1u : 0u;
-          wgmma_m64n64<1, 1, WG_F16>(d0, wg_desc_sw128(ah, Cpad * 128, 1024), db, acc);
-          wgmma_m64n64<1, 1, WG_F16>(d1, wg_desc_sw128(ah + Cpad * 128, Cpad * 128, 1024), db, acc);
-        }
-        const uint64_t dsx = wg_desc_sw128(smem_u32(sx0 + s * T4_SX_BYTES), 2048, 1024);
-        wgmma_m64n64<1, 1, WG_BF16>(d0, dqx0, dsx, 1u);
-        wgmma_m64n64<1, 1, WG_BF16>(d1, dqx1, dsx, 1u);
-        wg_commit();
+        const int s = h & (T4_STAGES - 1);
         wg_wait_all();
         mbar_arrive(&sm.stage_free[s]);                    // my part of the group's reads of the stage is done
-        t4_group_sync(g);                                  // the group has read the previous half-tile out of its stage
-        wg_store_m64n64(d0, accg, T4_ACC_LD, 0);
-        wg_store_m64n64(d1, accg, T4_ACC_LD, 64);
+        if (producer) produce(0);                          // this arrival may have been the stage's last
+        __syncwarp();
+        t4_group_sync(g);                                  // the group has read the previous tile out of its stage
+        wg_store_m64n32(d0, accg, T4_ACC_LD, 0);
+        wg_store_m64n32(d1, accg, T4_ACC_LD, 64);
         t4_group_sync(g);
+        if (h + 1 < H) mma(h + 1);
       }
-      // eight steps of 8 columns, two per iteration of a rolled loop (the flush code exists twice plus the final
+      // four steps of 8 columns, two per iteration of a rolled loop (the flush code exists twice plus the final
       // flush, not once per step: the instruction cache matters at ~700 instructions a copy)
 #pragma unroll 1
       for (int c8 = 0; c8 < T4_CT / 8; c8 += 2) {
@@ -334,9 +357,11 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
       }
     }
 #undef DGCN_T4_FILTER8
+    wg_wait_all();      // nothing is in flight (tile H - 1 started none); frees the accumulators for the epilogue
     flush();
     t4_group_sync(g);   // the group's wgmma have completed, nobody of the group reads its accumulator stage or flushes
-                        // any more: the stage and the candidate buffer become the work area
+                        // any more: the query plane with the stage behind it and the candidate buffer become the
+                        // work area
 
     const float cut = (lk[KP - 1] == 0xFFFFFFFFu) ? INFINITY : __uint_as_float(lk[KP - 1] & 0xFFFFF000u);
     const int C = a.C;
@@ -386,7 +411,7 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
       // hi = vK + delta(vK) + 2 eps  is beaten by K candidates (certainly OUT).  What lies in [lo, hi] is ranked by
       // the exact key (fp32 FMA chain, ties to the smaller index) and fills the remaining places.
       constexpr int MB = T4_MB;
-      uint64_t* band = reinterpret_cast<uint64_t*>(accg);               // [MB][TILE] exact keys
+      uint64_t* band = reinterpret_cast<uint64_t*>(gb);                 // [MB][TILE] exact keys
       const int K = a.K;
       float vK = INFINITY, vK1 = INFINITY;
 #pragma unroll
@@ -468,9 +493,9 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
       cta_epilogue_wide<4, false, true, 10>(a, b, q0, nullptr, sm.ok[g], sel, sel_ld, nullptr, 0, r);
     } else {
     // ---- exact re-rank of the listed candidates (fp32 FMA chain, channels ascending) --------------------------
-    uint64_t* list = reinterpret_cast<uint64_t*>(accg);                     // [KP][TILE]
+    uint64_t* list = reinterpret_cast<uint64_t*>(gb);                       // [KP][TILE]
     {
-      // Parts of at most 10 candidates (register budget of a 9-warp CTA at one CTA per SM).  Channels in chunks of 8 in
+      // Parts of at most 10 candidates (register budget of a 16-warp CTA at one CTA per SM).  Channels in chunks of 8 in
       // the outer loop, candidates in the inner one: HN independent FMA chains in flight; per candidate the chain is
       // acc = fma(x_q[c], x_j[c], acc) for c ascending from acc = 0 - the bits of the fp32 kernel.
       constexpr int PARTS = KP > 20 ? 4 : 2;
@@ -536,7 +561,6 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
     t4_group_sync(g);
     // ---- consumer: sel lives in the group's candidate buffer ---------------------------------------------------
     cta_epilogue_wide<4, false, false, 10>(a, b, q0, list, sm.ok[g], sel, sel_ld, nullptr, 0, r);
-    }
     }
   }
 }

@@ -1,13 +1,16 @@
 #!/usr/bin/env python
 """How much of knn_tc4_kernel's time follows its tensor-core work: time the headline layer's selection at
-C in {16, 32, 48, 64} and fit kernel ms against the m64n64k16 wgmma count per half-tile and filter warpgroup.
+C in {16, 32, 48, 64} and fit kernel ms against the wgmma count per candidate tile and filter warpgroup.
 
-    python tools/knn_tc4_cpad_sweep.py [--products 1|3] [--rounds R] [--steps S]
+    python tools/knn_tc4_cpad_sweep.py [--products 1|3] [--tile 32|64] [--rounds R] [--steps S]
 
 Workload: DynConv2d(C, 64, k=20, d=1, edge, relu, batch).eval() forward, B=16, N=4096 - the set-only consumer of
 bench.py's layer.  Only the channel count changes, so the filter, flush and consumer work stays (nearly) the same
-while the wgmma count per half-tile per group is 2 (P C/16 + 1): P = 1 for the single fp16 product, P = 3 for the
-three-product bf16 split (hi*hi, hi*mid, mid*hi).  --products names the scheme of the build being measured.
+while the wgmma count per candidate tile per group is 2 (P C/16 + 1): P = 1 for the single fp16 product, P = 3 for
+the three-product bf16 split (hi*hi, hi*mid, mid*hi).  --products names the scheme of the build being measured,
+--tile its candidate tile: 32 (m64n32k16 wgmma, four groups per CTA) or 64 (m64n64k16 per half-tile, the two-group
+builds before).  Either way one wgmma of the count is the same tensor work per candidate, so s and t0 of the two
+tile widths compare directly.
 
 Kernel time is the "knn" bracket of _native.kernel_timing (the selection kernel and its exact completion kernel,
 CUDA events on the launch stream), inputs rotate over 8 seeded batches, the configurations are alternated within
@@ -28,7 +31,7 @@ CHANNELS = (16, 32, 48, 64)
 N_ROTATE = 8
 
 
-def wgmma_per_half_tile(c, products):
+def wgmma_per_tile(c, products):
     return 2 * (products * ((c + 15) // 16) + 1)
 
 
@@ -50,6 +53,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--products", type=int, default=1, choices=(1, 3),
                     help="tensor-core products per channel block of the build measured (1: fp16, 3: bf16 split)")
+    ap.add_argument("--tile", type=int, default=32, choices=(32, 64),
+                    help="candidates per tile of the build measured (32: m64n32k16 wgmma, 64: m64n64k16)")
     ap.add_argument("--rounds", type=int, default=7)
     ap.add_argument("--steps", type=int, default=16)
     args = ap.parse_args()
@@ -98,13 +103,14 @@ def main():
         finally:
             _native.tc_certification(False)
 
-    x = np.array([wgmma_per_half_tile(c, args.products) for c in CHANNELS], dtype=np.float64)
+    x = np.array([wgmma_per_tile(c, args.products) for c in CHANNELS], dtype=np.float64)
     med = np.array([float(np.median(times[c])) for c in CHANNELS])
     s, t0 = np.polyfit(x, med, 1)
     pred_fp16, pred_bf16 = t0 + 10 * s, t0 + 26 * s
     out = {
-        "what": "knn_tc4_kernel + completion kernel ms per launch vs m64n64k16 wgmma per half-tile per group",
-        "products": args.products, "rounds": args.rounds, "steps_per_round": args.steps,
+        "what": "knn_tc4_kernel + completion kernel ms per launch vs m64n%dk16 wgmma per %d-candidate tile per group"
+                % (args.tile, args.tile),
+        "products": args.products, "tile": args.tile, "rounds": args.rounds, "steps_per_round": args.steps,
         "device": device_info(),
         "points": [{"C": c, "wgmma": int(w), "kernel_ms_median": m, "kernel_ms_min": min(times[c]),
                     "kernel_ms_max": max(times[c])} for c, w, m in zip(CHANNELS, x, med)],

@@ -75,16 +75,24 @@ __device__ __forceinline__ float pre_keep(float s, float t, float x, bool relu, 
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 static inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
-// Bump allocator over the caller-owned workspace.
+// Bump allocator over the caller-owned workspace.  A Workspace made without arguments only counts: take()
+// advances `off` as it would and returns nullptr, so a *_workspace_bytes() query is the launch's own carve run
+// this way, and a carve takes every region of a path before the path's first launch.
 struct Workspace {
   char* base;
   size_t size;
   size_t off;
   bool ok;
-  Workspace(void* p, size_t n) : base(static_cast<char*>(p)), size(n), off(0), ok(true) {}
+  bool counting;
+  Workspace() : base(nullptr), size(0), off(0), ok(true), counting(true) {}
+  Workspace(void* p, size_t n) : base(static_cast<char*>(p)), size(n), off(0), ok(true), counting(false) {}
   template <typename T>
   T* take(size_t count) {
     size_t bytes = align_up(count * sizeof(T), 256);
+    if (counting) {
+      off += bytes;
+      return nullptr;
+    }
     if (base == nullptr || off + bytes > size) {
       ok = false;
       return nullptr;

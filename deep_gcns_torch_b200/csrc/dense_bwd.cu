@@ -400,29 +400,40 @@ __global__ void mr_scatter_kernel(const float* __restrict__ dxcat, const int32_t
   atomicAdd(row + arg_i[t], -dr);
 }
 
-struct BwdPlan {
-  size_t wk, bk, pq, dpq, partial, sums, dwcat, sf, xt, r, argj, argi, z, dxcat;
-  int64_t n_partial;
+// The regions of dgcn_graph_conv_backward_sync, in the order it uses them.
+struct BwdRegions {
+  int64_t n_partial;         // statistic rows: one per CTA of edge_bwd_kernel / mr_bn_bwd_kernel
+  float* wk;                 // packed weights
+  float* partial;            // [n_partial][3][co] partial sums
+  double* sums;              // [3][co] their fixed-order reductions
+  float *bk, *pq, *dpq;      // EdgeConv: packed bias, node GEMM (B,N,2co), its gradient (B,2co,N)
+  float* dwcat;              // EdgeConv: dWcat (2co x ci), first the transposed weights for grad_x
+  float* sf;                 // EdgeConv, train mode: (dbeta, dgamma) as floats for pass 1
+  float *xt, *r, *z, *dxcat; // MRConv: node-major copy of x, max_j x_j - x_i, z then dz, d[x; r]
+  int32_t *argj, *argi;      // MRConv: arg-max neighbour and its centre per (b, c, i)
 };
-static BwdPlan bwd_plan(int conv, int64_t B, int64_t ci, int64_t co, int64_t N) {
-  BwdPlan p{};
-  p.sums = 3 * co * 2;   // doubles, counted in floats
-  if (conv == DGCN_CONV_EDGE) {
-    p.wk = ci * 2 * co; p.bk = 2 * co; p.pq = B * N * 2 * co; p.dpq = B * 2 * co * N;
-    p.n_partial = ceil_div(N, 32) * B; p.partial = p.n_partial * 3 * co; p.dwcat = 2 * co * ci;
-    p.sf = 2 * co;   // train-mode BN: (dbeta, dgamma) as floats for pass B
+static BwdRegions carve_bwd(int conv, int64_t B, int64_t ci, int64_t co, int64_t N, bool train, Workspace& ws) {
+  BwdRegions r{};
+  const bool edge = conv == DGCN_CONV_EDGE;
+  r.n_partial = edge ? ceil_div(N, 32) * B : ceil_div(N, 256) * B;
+  r.wk = ws.take<float>(2 * ci * co);
+  r.partial = ws.take<float>(r.n_partial * 3 * co);
+  r.sums = ws.take<double>(3 * co);
+  if (edge) {
+    r.bk = ws.take<float>(2 * co);
+    r.pq = ws.take<float>(B * N * 2 * co);
+    r.dpq = ws.take<float>(B * 2 * co * N);
+    r.dwcat = ws.take<float>(2 * co * ci);
+    r.sf = train ? ws.take<float>(2 * co) : nullptr;
   } else {
-    p.wk = 2 * ci * co; p.xt = B * N * ci; p.r = B * ci * N; p.argj = B * ci * N; p.argi = B * ci * N;
-    p.z = B * co * N; p.dxcat = B * 2 * ci * N;
-    p.n_partial = ceil_div(N, 256) * B; p.partial = p.n_partial * 3 * co;
+    r.xt = ws.take<float>(B * N * ci);
+    r.r = ws.take<float>(B * ci * N);
+    r.argj = ws.take<int32_t>(B * ci * N);
+    r.argi = ws.take<int32_t>(B * ci * N);
+    r.z = ws.take<float>(B * co * N);
+    r.dxcat = ws.take<float>(B * 2 * ci * N);
   }
-  return p;
-}
-static size_t bwd_plan_bytes(const BwdPlan& p) {
-  size_t b = 0;
-  for (size_t v : {p.wk, p.bk, p.pq, p.dpq, p.partial, p.sums, p.dwcat, p.sf, p.xt, p.r, p.argj, p.argi, p.z, p.dxcat})
-    b += align_up(v * 4, 256);
-  return b + 512;
+  return r;
 }
 
 }  // namespace dgcn
@@ -434,7 +445,9 @@ extern "C" {
 size_t dgcn_graph_conv_backward_workspace_bytes(int32_t conv, int64_t B, int64_t C_in, int64_t C_out, int64_t N,
                                                 int64_t k) {
   (void)k;
-  return bwd_plan_bytes(bwd_plan(conv, B, C_in, C_out, N));
+  Workspace ws;
+  carve_bwd(conv, B, C_in, C_out, N, true, ws);   // train mode carves the most
+  return ws.off + 512;   // 512 bytes past the last region; nothing is placed there
 }
 
 int dgcn_graph_conv_backward(int32_t conv, const float* x, int64_t B, int64_t ci, int64_t N, int64_t sb, int64_t sc,
@@ -461,24 +474,20 @@ int dgcn_graph_conv_backward_sync(int32_t conv, const float* x, int64_t B, int64
   if (B > 65535 || co > 65535) return DGCN_ERR_UNSUPPORTED;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   Workspace ws(wsp, ws_bytes);
-  BwdPlan pl = bwd_plan(conv, B, ci, co, N);
   const int vec = ((reinterpret_cast<uintptr_t>(x) & 15) == 0 && sb % 4 == 0 && sc % 4 == 0 && N % 4 == 0) ? 1 : 0;
   const bool train = p->norm == DGCN_NORM_BATCH_TRAIN;
   if (!train) sync = nullptr;
   const float slope = act_slope_of(p);
   const float* prelu = p->act == DGCN_ACT_PRELU ? p->prelu_weight : nullptr;
-  float* wk = ws.take<float>(pl.wk);
-  float* partial = ws.take<float>(pl.partial);
-  double* sums = reinterpret_cast<double*>(ws.take<float>(pl.sums));
+  const BwdRegions w = carve_bwd(conv, B, ci, co, N, train, ws);
   if (!ws.ok) return DGCN_ERR_WORKSPACE;
+  float* wk = w.wk;
+  float* partial = w.partial;
+  double* sums = w.sums;
   const int iN = static_cast<int>(N), ico = static_cast<int>(co), ici = static_cast<int>(ci), iB = static_cast<int>(B);
 
   if (conv == DGCN_CONV_EDGE) {
-    float* bk = ws.take<float>(pl.bk);
-    float* pq = ws.take<float>(pl.pq);
-    float* dpq = ws.take<float>(pl.dpq);
-    float* dwcat = ws.take<float>(pl.dwcat);
-    if (!ws.ok) return DGCN_ERR_WORKSPACE;
+    float *bk = w.bk, *pq = w.pq, *dpq = w.dpq, *dwcat = w.dwcat;
     const int M = 2 * ico;
     pack_edge_weights_kernel<<<static_cast<unsigned>(ceil_div(ci * M, 256)), 256, 0, stream>>>(p->weight, p->bias, ici,
                                                                                              ico, wk, bk);
@@ -486,7 +495,7 @@ int dgcn_graph_conv_backward_sync(int32_t conv, const float* x, int64_t B, int64
     node_pq_kernel<<<dim3(ceil_div(M, TILE), ceil_div(N, TILE), B), NTHREADS, 0, stream>>>(x, sb, sc, ici, iN, vec, wk, bk,
                                                                                          M, pq);
     DGCN_LAUNCH_CHECK();
-    DGCN_CUDA_TRY(cudaMemsetAsync(dpq, 0, pl.dpq * 4, stream));
+    DGCN_CUDA_TRY(cudaMemsetAsync(dpq, 0, static_cast<size_t>(B) * M * N * sizeof(float), stream));
     EdgeBwdArgs g{};
     g.pq = pq; g.edge_index = edge_index; g.nbr = nbr; g.B = iB; g.N = iN; g.k = static_cast<int>(k); g.co = ico;
     g.slope = slope; g.prelu = prelu; g.norm = p->norm;
@@ -498,22 +507,18 @@ int dgcn_graph_conv_backward_sync(int32_t conv, const float* x, int64_t B, int64
     if (train) {
       edge_bwd_kernel<0><<<grid, 256, 0, stream>>>(g);
       DGCN_LAUNCH_CHECK();
-      int rc = bn_bwd_pass0_sums(partial, pl.n_partial, ico, static_cast<double>(B) * N * k, sync, sums, &g1.inv_count,
+      int rc = bn_bwd_pass0_sums(partial, w.n_partial, ico, static_cast<double>(B) * N * k, sync, sums, &g1.inv_count,
                                  stream);
       if (rc != DGCN_OK) return rc;
-    }
-    if (train) {
       // pass B wants (dbeta, dgamma) as float[2][co]: finish_param_grads_kernel does the conversion
-      float* sf = ws.take<float>(pl.sf);
-      if (!ws.ok) return DGCN_ERR_WORKSPACE;
-      finish_param_grads_kernel<<<static_cast<unsigned>(ceil_div(co, 128)), 128, 0, stream>>>(sums, ico, 0, sf + co, sf,
-                                                                                           nullptr);
+      finish_param_grads_kernel<<<static_cast<unsigned>(ceil_div(co, 128)), 128, 0, stream>>>(sums, ico, 0, w.sf + co,
+                                                                                           w.sf, nullptr);
       DGCN_LAUNCH_CHECK();
-      g1.sums = sf;
+      g1.sums = w.sf;
     }
     edge_bwd_kernel<1><<<grid, 256, 0, stream>>>(g1);
     DGCN_LAUNCH_CHECK();
-    reduce_partials_kernel<<<dim3(ico, 3), 256, 0, stream>>>(partial, pl.n_partial, 3, ico, sums);
+    reduce_partials_kernel<<<dim3(ico, 3), 256, 0, stream>>>(partial, w.n_partial, 3, ico, sums);
     DGCN_LAUNCH_CHECK();
     finish_param_grads_kernel<<<static_cast<unsigned>(ceil_div(co, 128)), 128, 0, stream>>>(
         sums, ico, prelu != nullptr, p->norm != DGCN_NORM_NONE ? grad_bn_weight : nullptr,
@@ -531,7 +536,7 @@ int dgcn_graph_conv_backward_sync(int32_t conv, const float* x, int64_t B, int64
       DGCN_LAUNCH_CHECK();
     }
     if (grad_weight) {
-      DGCN_CUDA_TRY(cudaMemsetAsync(dwcat, 0, pl.dwcat * 4, stream));
+      DGCN_CUDA_TRY(cudaMemsetAsync(dwcat, 0, static_cast<size_t>(M) * ci * sizeof(float), stream));
       const int tiles = static_cast<int>(ceil_div(M, TILE) * ceil_div(ci, TILE));
       wgrad_kernel<<<dim3(ceil_div(N, KCH), tiles, B), NTHREADS, 0, stream>>>(dpq, static_cast<int64_t>(M) * N, N, M, x,
                                                                             sb, sc, ici, iN, dwcat, ci);
@@ -548,13 +553,8 @@ int dgcn_graph_conv_backward_sync(int32_t conv, const float* x, int64_t B, int64
   }
 
   // ---- MRConv ---------------------------------------------------------------------------------------------
-  float* xt = ws.take<float>(pl.xt);
-  float* r = ws.take<float>(pl.r);
-  int32_t* argj = ws.take<int32_t>(pl.argj);
-  int32_t* argi = ws.take<int32_t>(pl.argi);
-  float* z = ws.take<float>(pl.z);
-  float* dxcat = ws.take<float>(pl.dxcat);
-  if (!ws.ok) return DGCN_ERR_WORKSPACE;
+  float *xt = w.xt, *r = w.r, *z = w.z, *dxcat = w.dxcat;
+  int32_t *argj = w.argj, *argi = w.argi;
   to_node_major_kernel<<<dim3(ceil_div(N, 32), ceil_div(ci, 32), B), dim3(32, 8), 0, stream>>>(x, sb, sc, ici, iN, xt);
   DGCN_LAUNCH_CHECK();
   MrGatherArgs mg{xt, edge_index, nbr, iB, iN, static_cast<int>(k), ici, r, argj, argi};
@@ -589,12 +589,12 @@ int dgcn_graph_conv_backward_sync(int32_t conv, const float* x, int64_t B, int64
   if (train) {
     mr_bn_bwd_kernel<0><<<bgrid, 256, 0, stream>>>(mb);
     DGCN_LAUNCH_CHECK();
-    int rc = bn_bwd_pass0_sums(partial, pl.n_partial, ico, static_cast<double>(B) * N, sync, sums, &mb.inv_count, stream);
+    int rc = bn_bwd_pass0_sums(partial, w.n_partial, ico, static_cast<double>(B) * N, sync, sums, &mb.inv_count, stream);
     if (rc != DGCN_OK) return rc;
   }
   mr_bn_bwd_kernel<1><<<bgrid, 256, 0, stream>>>(mb);   // z now holds dz
   DGCN_LAUNCH_CHECK();
-  reduce_partials_kernel<<<dim3(ico, 3), 256, 0, stream>>>(partial, pl.n_partial, 3, ico, sums);
+  reduce_partials_kernel<<<dim3(ico, 3), 256, 0, stream>>>(partial, w.n_partial, 3, ico, sums);
   DGCN_LAUNCH_CHECK();
   finish_param_grads_kernel<<<static_cast<unsigned>(ceil_div(co, 128)), 128, 0, stream>>>(
       sums, ico, prelu != nullptr, p->norm != DGCN_NORM_NONE ? grad_bn_weight : nullptr,

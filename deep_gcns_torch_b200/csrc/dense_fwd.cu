@@ -4,7 +4,6 @@
 #include <stdlib.h>
 #include <string.h>
 #include <stdio.h>
-#include <stdlib.h>
 #include "knn_tc4.cuh"
 
 namespace dgcn {
@@ -16,47 +15,173 @@ int dist_rows_tc_prepare(const KnnArgs& a, __nv_bfloat16* planes, cudaStream_t s
 int dist_rows_tc_launch(const KnnArgs& a, const __nv_bfloat16* planes, int b0, int nb, float* drows, int ldd,
                         cudaStream_t stream);
 
-__global__ void to_node_major_kernel(const float* __restrict__ x, int64_t sb, int64_t sc, int C, int N,
-                                     float* __restrict__ xt);
-
-// ---- launch helpers for the selection kernels -------------------------------------
-// Clouds per slab of distance rows: two slabs are in flight (rows of slab s+1 under the select of slab s), so each
-// gets half of the L2 (at least one cloud).
-static size_t knn_slab_clouds(int64_t B, int64_t N) {
-  const int64_t ldd = (N + 3) / 4 * 4;
-  const int64_t per_cloud = N * ldd * 4;
-  int64_t nb = static_cast<int64_t>(device_l2_bytes() / 2) / (per_cloud > 0 ? per_cloud : 1);
-  if (nb < 1) nb = 1;
-  if (nb > B) nb = B;
-  return static_cast<size_t>(nb);
-}
-
+// ---- kNN plan: the route of a call, decided once -------------------------------------
 constexpr int TC_FALLBACK_GRID = 132;  // CTAs of the exact completion kernel (one uncertified query at a time each; H100 SXM SMs)
 
-static bool tc_shape_ok(int64_t C, int64_t N, int64_t K) {
-  return K <= TC_K_MAX && C <= TC_MAX_C && N >= TILE && (N % TILE) == 0;
+// The device limits a plan reads, read once per call so that the workspace query and the launch see the same values.
+struct DeviceLimits { int sms; size_t l2_bytes; };
+static DeviceLimits device_limits() { return DeviceLimits{device_sm_count(), device_l2_bytes()}; }
+
+static int next_pow2(int v) {
+  int p = 1;
+  while (p < v) p <<= 1;
+  return p;
 }
 
-size_t knn_workspace_bytes(int64_t B, int64_t C, int64_t N, int64_t K) {
-  size_t bytes = align_up(static_cast<size_t>(B) * N * 4, 256);
-  if (tc_shape_ok(C, N, K)) {
-    const int64_t cpad = (C + 15) / 16 * 16;
-    bytes += align_up(static_cast<size_t>(B) * TC_PLANES * cpad * N * 2, 256);   // bf16 planes
-    bytes += align_up(static_cast<size_t>(B) * N * C * 4, 256);          // node-major copy
-    bytes += align_up(static_cast<size_t>(B) * 8, 256);                  // per-cloud max |x|^2, max fp16 rounding error
-    bytes += align_up(static_cast<size_t>(B) * 8 * N * 2, 256);          // -|x|^2/2 operand block
-    bytes += align_up(static_cast<size_t>(B) * N * 4 + 256, 256);        // fail counter + list
+enum KnnRoute {
+  KNN_SMALL,   // knn_small_kernel: fp32 distance tiles, K <= SMALL_K_MAX
+  KNN_TC,      // tensor-core pre-filter (knn_tc_kernel or knn_tc4_kernel) + exact completion, K <= TC_K_MAX
+  KNN_SLAB     // distance rows of a slab of clouds in the workspace + one warp per row, K <= LARGE_K_MAX
+};
+
+struct KnnPlan {
+  KnnRoute route;
+  int64_t n_partial;   // train-mode statistic rows the route's EdgeConv epilogue writes
+  dim3 grid;           // query tiles x clouds
+  int kp, kp4;         // KNN_TC: list lengths of knn_tc_kernel and knn_tc4_kernel
+  bool packed;         // KNN_TC: knn_tc_kernel's packed candidate keys (N <= 4096)
+  bool tc4;            // KNN_TC: knn_tc4_kernel, provided the carved rows turn out aligned for it
+  bool rows_on_tc;     // KNN_SLAB: distance rows on the tensor cores (dist_rows_tc.cu), else dist_rows_kernel
+  bool two_slabs;      // KNN_SLAB: a second slab buffer, the distance rows of slab s+1 run under the select of slab s
+  bool fast;           // KNN_SLAB: select_rows_fast_kernel first, handing the rows it cannot finish to the exact select
+  int nbmax, ldd;      // KNN_SLAB: clouds per slab, distance row stride
+  int KP, warps, cap, sample_rank, warps_f, select_grid;   // KNN_SLAB: select parameters
+  size_t smem, smem_f;
+};
+
+// The one place that decides how a call selects.  Host arithmetic on the shape, k, the flags and the epilogue's
+// mode: nothing here reads a pointer, so a workspace query plans exactly as the launch does.  Returns
+// DGCN_ERR_UNSUPPORTED for a slab the kernels do not cover (the plan is filled in all the same).
+static int knn_plan(const KnnArgs& a, const DeviceLimits& lim, KnnPlan& p) {
+  const int B = a.B, C = a.C, N = a.N, K = a.K;
+  p = KnnPlan{};
+  p.grid = dim3(static_cast<unsigned>(ceil_div(N, TILE)), B);
+  const int64_t n_cta = static_cast<int64_t>(p.grid.x) * p.grid.y;
+  const bool train = a.epi.mode == EPI_EDGE && a.epi.norm == DGCN_NORM_BATCH_TRAIN;
+  const bool tc_shape = C <= TC_MAX_C && N >= TILE && (N % TILE) == 0;
+  if (!a.exact_fp32 && tc_shape && K <= TC_K_MAX && a.k <= SEL_LD && !(train && a.epi.c_out > 128)) {
+    p.route = KNN_TC;
+    p.n_partial = n_cta + TC_FALLBACK_GRID;   // knn_exact_rows_kernel writes one row per CTA
+    // list length = K + certification margin
+    // (a margin of 4 ranks leaves ~1e-5 of the queries of a random 64-d cloud uncertified, 8 ranks none)
+    p.kp = K <= 9 ? 16 : K <= 20 ? 28 : K <= 32 ? 40 : 56;
+    p.kp4 = knn_tc4_list_len(K);
+    p.packed = N <= 4096;
+    // T4_GROUPS query tiles per CTA, warp specialised (knn_tc4.cuh), where its smaller work area and fixed consumer fit
+    p.tc4 = !a.tc_tile_per_cta && p.packed && !train && (C & 7) == 0 && knn_tc4_list_ok(p.kp4, a.k);
+    return DGCN_OK;
   }
-  if (K > SMALL_K_MAX) {
-    const int64_t ldd = (N + 3) / 4 * 4;
-    const size_t nslab = static_cast<size_t>(B) > knn_slab_clouds(B, N) ? 2 : 1;   // two slabs: distance rows of slab s+1 overlap the select of slab s
-    bytes += nslab * align_up(knn_slab_clouds(B, N) * N * ldd * 4, 256);
-    bytes += nslab * align_up(knn_slab_clouds(B, N) * N * 4 + 256, 256);   // rows the sampled select hands to the exact kernel (one list per slab buffer)
-    if (C <= TC_MAX_C && N >= TILE && N % TILE == 0) bytes += align_up(dist_rows_tc_plane_elems(B, C, N) * 2, 256);   // (hi, mid, lo) planes
+  if (K <= SMALL_K_MAX) {
+    p.route = KNN_SMALL;
+    p.n_partial = n_cta;
+    return DGCN_OK;
   }
-  return bytes + 256;
+  p.route = KNN_SLAB;
+  p.n_partial = static_cast<int64_t>(B) * N;
+  p.rows_on_tc = K <= LARGE_K_MAX && dist_rows_tc_ok(a);
+  p.ldd = (N + 3) / 4 * 4;
+  // Clouds per slab of distance rows: two slabs are in flight (rows of slab s+1 under the select of slab s), so each
+  // gets half of the L2 (at least one cloud).
+  const int64_t per_cloud = static_cast<int64_t>(N) * p.ldd * 4;
+  int64_t nb = static_cast<int64_t>(lim.l2_bytes / 2) / (per_cloud > 0 ? per_cloud : 1);
+  if (nb < 1) nb = 1;
+  if (nb > B) nb = B;
+  p.nbmax = static_cast<int>(nb);
+  p.two_slabs = B > p.nbmax;
+  p.KP = next_pow2(K);
+  const size_t per_warp = static_cast<size_t>(p.KP) * 8 + static_cast<size_t>(p.ldd) * 4 + static_cast<size_t>((a.k + 31) / 32 * 32) * 4;   // ldd = N rounded up to 4 keeps every warp's u64 array 16-byte aligned
+  p.warps = static_cast<int>((200u << 10) / per_warp);   // 0: a single row does not fit in shared memory
+  if (p.warps > 4) p.warps = 4;
+  p.smem = per_warp * p.warps;
+  // sampled fast select: bound = sample_rank-th of 128 samples (mean + 2.5 sigma + 2 of the K/N quantile)
+  const double pq = static_cast<double>(K) / N;
+  p.sample_rank = static_cast<int>(128.0 * pq + 2.5 * sqrt(128.0 * pq * (1.0 - pq)) + 2.0) + 1;
+  if (p.sample_rank > 127) p.sample_rank = 127;
+  // room for every key below the bound (no power of two needed: only the wanted bins get sorted);
+  // k > 64 keeps the full sort and needs the padded power of two
+  // keys below a bound at sample rank r: mean (r+1)/129 N, relative spread ~ 1/sqrt(r+1); leave 3.5 sigma
+  const double wmean = (p.sample_rank + 1) / 129.0 * N;
+  const int64_t wcap = static_cast<int64_t>(wmean * (1.0 + 3.5 / sqrt(p.sample_rank + 1.0))) + 32;
+  int cap = static_cast<int>(wcap > K + 64 ? wcap : K + 64);
+  cap = a.k > 64 ? next_pow2(cap > 2 * K ? cap : 2 * K) : (cap + 31) / 32 * 32;
+  if (cap < 128) cap = 128;            // the sorted sample lives in the same array
+  if (cap > 2048) cap = 2048;
+  p.cap = cap;
+  p.fast = N >= 512 && cap >= K;
+  const size_t per_warp_f = static_cast<size_t>(cap) * 8 + static_cast<size_t>((a.k + 31) / 32 * 32) * 4 + 2560;   // keys, sel, multi-select tables (hist 256, prefix 260 ints, 256 marks -> 2320 B)
+  p.warps_f = static_cast<int>((56u << 10) / per_warp_f);   // <= 56 KB per CTA: four CTAs per SM
+  if (p.warps_f > 8) p.warps_f = 8;
+  if (p.warps_f < 1) p.warps_f = 1;
+  p.smem_f = per_warp_f * p.warps_f;
+  p.select_grid = 2 * lim.sms;   // grid-stride over the rows the fast select hands over
+  return K > LARGE_K_MAX || p.warps < 1 ? DGCN_ERR_UNSUPPORTED : DGCN_OK;
 }
 
+// the fused prologue can also produce PQ (EdgeConv): channel / output counts it supports
+static bool prologue_pq_ok(const KnnPlan& p, int64_t M) {
+  return p.route == KNN_TC && M % 128 == 0 && M <= 256;
+}
+
+// ---- kNN workspace: one carve per route ------------------------------------------------
+struct KnnRegions {
+  float* sq;                     // (B,N) squared norms
+  __nv_bfloat16 *planes, *sqp;   // KNN_TC: operand planes, -|x|^2/2 operand block
+  float *xt_own, *sqmax;         // KNN_TC: node-major copy of x (MRConv brings its own), max |x|^2 and fp16 error per cloud
+  int* fail;                     // KNN_TC: uncertified queries, a counter (first 64 ints) then the list
+  __nv_bfloat16* planes3;        // KNN_SLAB: (hi, mid, lo) planes of the tensor-core distance rows
+  float* drows[2];               // KNN_SLAB: distance rows, one buffer per slab in flight
+  int* rowlist[2];               // KNN_SLAB: per buffer, a counter (first 64 ints) then the rows the fast select hands over
+};
+
+static void carve_knn_tc(const KnnArgs& a, Workspace& ws, KnnRegions& r) {
+  const size_t B = a.B, N = a.N, cpad = (a.C + 15) / 16 * 16;
+  r.planes = ws.take<__nv_bfloat16>(B * TC_PLANES * cpad * N);
+  r.xt_own = a.epi.mode == EPI_MR ? nullptr : ws.take<float>(B * N * a.C);
+  r.sqmax = ws.take<float>(B * 2);
+  r.sqp = ws.take<__nv_bfloat16>(B * 8 * N);
+  r.fail = ws.take<int>(B * N + 64);
+}
+
+static void carve_knn_slab(const KnnArgs& a, const KnnPlan& p, Workspace& ws, KnnRegions& r) {
+  if (p.rows_on_tc) r.planes3 = ws.take<__nv_bfloat16>(dist_rows_tc_plane_elems(a.B, a.C, a.N));
+  const int nbuf = p.two_slabs ? 2 : 1;
+  for (int i = 0; i < nbuf; ++i) r.drows[i] = ws.take<float>(static_cast<size_t>(p.nbmax) * a.N * p.ldd);
+  if (p.fast)
+    for (int i = 0; i < nbuf; ++i) r.rowlist[i] = ws.take<int>(static_cast<size_t>(p.nbmax) * a.N + 64);
+}
+
+static KnnRegions carve_knn(const KnnArgs& a, const KnnPlan& p, Workspace& ws) {
+  KnnRegions r{};
+  r.sq = ws.take<float>(static_cast<size_t>(a.B) * a.N);
+  if (p.route == KNN_TC) carve_knn_tc(a, ws, r);
+  if (p.route == KNN_SLAB) carve_knn_slab(a, p, ws, r);
+  return r;
+}
+
+// Largest carve over every route a call of this shape can take.  Besides the shape, the route depends on
+// DGCN_KNN_EXACT_FP32, on train-mode BatchNorm (for the EdgeConv epilogue) and on k; `carve` is run in counting
+// mode for each combination.
+template <typename Carve>
+static size_t max_over_routes(int64_t B, int64_t C, int64_t N, int64_t K, int mode, int64_t c_out, Carve carve) {
+  KnnArgs a{};
+  a.B = static_cast<int>(B); a.C = static_cast<int>(C); a.N = static_cast<int>(N); a.K = static_cast<int>(K);
+  a.epi.mode = mode; a.epi.c_in = a.C; a.epi.c_out = static_cast<int>(c_out);
+  const DeviceLimits lim = device_limits();
+  size_t most = 0;
+  for (int exact = 0; exact < 2; ++exact)
+    for (int norm : {DGCN_NORM_NONE, DGCN_NORM_BATCH_TRAIN})
+      for (int k : {1, a.K}) {
+        a.exact_fp32 = exact; a.epi.norm = norm; a.k = k;
+        KnnPlan p;
+        knn_plan(a, lim, p);   // an unsupported slab is still sized as planned
+        Workspace ws;
+        carve(a, p, ws);
+        if (ws.off > most) most = ws.off;
+      }
+  return most;
+}
+
+// ---- kNN launch ------------------------------------------------------------------------
 // Side stream of the large-K slab pipeline, one per device, created on first use (a write-once cache: the stream
 // carries no state between calls - every call forks it from and joins it back into the caller's stream by events).
 static cudaStream_t slab_side_stream() {
@@ -73,12 +198,6 @@ static cudaStream_t slab_side_stream() {
     }
   }
   return s;
-}
-
-static int next_pow2(int v) {
-  int p = 1;
-  while (p < v) p <<= 1;
-  return p;
 }
 
 // cuTensorMapEncodeTiled through the runtime (no link against libcuda): resolved once, the pointer is a
@@ -118,67 +237,55 @@ static int make_plane_map(CUtensorMap* map, const void* base, int64_t rows, int6
   return rc == CUDA_SUCCESS ? DGCN_OK : DGCN_ERR_CUDA;
 }
 
-// Tensor-core pre-filter path (knn_tc.cuh).  xt: node-major copy of x if the caller has one.
-static int launch_knn_tc(KnnArgs& a, Workspace& ws, cudaStream_t stream, const float* xt, int64_t* n_partial,
+// Tensor-core pre-filter route (knn_tc.cuh).
+static int launch_knn_tc(KnnArgs& a, const KnnPlan& pl, const KnnRegions& r, cudaStream_t stream,
                          const ProloguePq* pqf) {
-  const int B = a.B, N = a.N, C = a.C, K = a.K;
+  const int B = a.B, N = a.N, C = a.C;
   const int cpad = (C + 15) / 16 * 16;
-  __nv_bfloat16* planes = ws.take<__nv_bfloat16>(static_cast<size_t>(B) * TC_PLANES * cpad * N);
-  float* xt_own = xt ? nullptr : ws.take<float>(static_cast<size_t>(B) * N * C);
-  float* sqmax = ws.take<float>(static_cast<size_t>(B) * 2);   // max |x|^2, max fp16 rounding error |e|^2
-  __nv_bfloat16* sqp = ws.take<__nv_bfloat16>(static_cast<size_t>(B) * 8 * N);
-  int* fail = ws.take<int>(static_cast<size_t>(B) * N + 64);
-  if (!ws.ok) return DGCN_ERR_WORKSPACE;
-  DGCN_CUDA_TRY(cudaMemsetAsync(fail, 0, 256, stream));
-  DGCN_CUDA_TRY(cudaMemsetAsync(sqmax, 0, static_cast<size_t>(B) * 8, stream));
-  if (!xt) xt = xt_own;
+  DGCN_CUDA_TRY(cudaMemsetAsync(r.fail, 0, 256, stream));
+  DGCN_CUDA_TRY(cudaMemsetAsync(r.sqmax, 0, static_cast<size_t>(B) * 8, stream));
+  const float* xt = a.epi.mode == EPI_MR ? a.epi.xt : r.xt_own;
   // The kernel is chosen before the prologue: knn_tc4_kernel reads one fp16 plane, knn_tc_kernel the two bf16 planes.
-  // list length = K + certification margin
-  // (a margin of 4 ranks leaves ~1e-5 of the queries of a random 64-d cloud uncertified, 8 ranks none)
-  const int kp = K <= 9 ? 16 : K <= 20 ? 28 : K <= 32 ? 40 : 56;
-  const int kp4 = knn_tc4_list_len(K);
-  const bool packed = N <= 4096;
+  // Its alignment conditions are known only now that the regions are carved.
   const bool wide = epilogue_wide_ok(a);
   const bool xt32 = (reinterpret_cast<uintptr_t>(xt) & 31) == 0;
-  // T4_GROUPS query tiles per CTA, warp specialised (knn_tc4.cuh), where its smaller work area and fixed consumer fit
-  const bool train = a.epi.mode == EPI_EDGE && a.epi.norm == DGCN_NORM_BATCH_TRAIN;
-  const bool quad = !a.tc_tile_per_cta && packed && wide && !train && xt32 && (C & 7) == 0 && knn_tc4_list_ok(kp4, a.k);
+  const bool quad = pl.tc4 && wide && xt32;
   // sq, operand plane(s), node-major copy and max |x|^2 in one pass over x (sq overwrites what the caller computed)
   if (pqf) {   // the EdgeConv node GEMM rides on the same pass over x
     const size_t smem = (static_cast<size_t>(TC_MAX_C) * 68 + static_cast<size_t>(C) * pqf->M) * 4;
     DGCN_ENSURE_SMEM((tc_prologue_pq_kernel), smem);
     tc_prologue_pq_kernel<<<dim3(N / 64, B), 256, smem, stream>>>(a.x, a.sb, a.sc, C, cpad, N, const_cast<float*>(a.sq),
-                                                                  planes, xt_own, sqmax, sqp, *pqf, quad);
+                                                                  r.planes, r.xt_own, r.sqmax, r.sqp, *pqf, quad);
   } else {
     tc_prologue_kernel<<<dim3(ceil_div(N, 32), B), 256, 0, stream>>>(a.x, a.sb, a.sc, C, cpad, N,
-                                                                 const_cast<float*>(a.sq), planes,
-                                                                 xt_own, sqmax, sqp, quad);
+                                                                 const_cast<float*>(a.sq), r.planes,
+                                                                 r.xt_own, r.sqmax, r.sqp, quad);
   }
   DGCN_LAUNCH_CHECK();
   TcArgs t{};
   {
-    int rc = quad ? make_plane_map(&t.tm_planes, planes, static_cast<int64_t>(B) * cpad, N, 64, cpad,
+    int rc = quad ? make_plane_map(&t.tm_planes, r.planes, static_cast<int64_t>(B) * cpad, N, 64, cpad,
                                    CU_TENSOR_MAP_DATA_TYPE_FLOAT16)
-                  : make_plane_map(&t.tm_planes, planes, static_cast<int64_t>(B) * TC_PLANES * cpad, N, 64, cpad,
+                  : make_plane_map(&t.tm_planes, r.planes, static_cast<int64_t>(B) * TC_PLANES * cpad, N, 64, cpad,
                                    CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
     if (rc == DGCN_OK)
-      rc = make_plane_map(&t.tm_sqp, sqp, static_cast<int64_t>(B) * 8, N, 64, 8, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
+      rc = make_plane_map(&t.tm_sqp, r.sqp, static_cast<int64_t>(B) * 8, N, 64, 8, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
     if (quad && rc == DGCN_OK)   // knn_tc4_kernel's 32-candidate tiles
-      rc = make_plane_map(&t.tm_cand, planes, static_cast<int64_t>(B) * cpad, N, T4_CT, cpad, CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
+      rc = make_plane_map(&t.tm_cand, r.planes, static_cast<int64_t>(B) * cpad, N, T4_CT, cpad, CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
     if (quad && rc == DGCN_OK)
-      rc = make_plane_map(&t.tm_sqc, sqp, static_cast<int64_t>(B) * 8, N, T4_CT, 8, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
+      rc = make_plane_map(&t.tm_sqc, r.sqp, static_cast<int64_t>(B) * 8, N, T4_CT, 8, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
     if (rc != DGCN_OK) return rc;
   }
   t.a = a;
-  t.planes = planes;
-  t.sqp = sqp;
+  t.planes = r.planes;
+  t.sqp = r.sqp;
   t.xt = xt;
   t.xt32 = xt32 ? 1 : 0;
-  t.sqmax = sqmax;
+  t.sqmax = r.sqmax;
   t.Cpad = cpad;
-  t.fail_count = fail;
-  t.fail_list = fail + 64;
-  const dim3 grid(N / TILE, B);
+  t.fail_count = r.fail;
+  t.fail_list = r.fail + 64;
+  const dim3 grid = pl.grid;
   const int64_t n_cta = static_cast<int64_t>(grid.x) * grid.y;
   {
     KernelTimer timer(stream, "knn");
@@ -186,17 +293,17 @@ static int launch_knn_tc(KnnArgs& a, Workspace& ws, cudaStream_t stream, const f
     t.wide = wide ? 1 : 0;
     t.flush_early = TC_FLUSH_EARLY;
     t.flush_late = TC_FLUSH_LATE;
-    t.work_bytes = static_cast<int>(tc_work_bytes(kp, a.k, t.wide != 0, nch));
+    t.work_bytes = static_cast<int>(tc_work_bytes(pl.kp, a.k, t.wide != 0, nch));
     const size_t smem = static_cast<size_t>(t.work_bytes) + sizeof(TcTail) + 1024;
     int rc;
     if (quad) {
-      rc = launch_knn_tc4(kp4, t, dim3(static_cast<unsigned>(ceil_div(N / TILE, T4_GROUPS)), B), stream);
+      rc = launch_knn_tc4(pl.kp4, t, dim3(static_cast<unsigned>(ceil_div(N / TILE, T4_GROUPS)), B), stream);
     } else
-    switch (kp) {
-      case 16: rc = launch_knn_tc_kp16(packed, t, grid, smem, stream); break;
-      case 28: rc = launch_knn_tc_kp28(packed, t, grid, smem, stream); break;
-      case 40: rc = launch_knn_tc_kp40(packed, t, grid, smem, stream); break;
-      default: rc = launch_knn_tc_kp56(packed, t, grid, smem, stream); break;
+    switch (pl.kp) {
+      case 16: rc = launch_knn_tc_kp16(pl.packed, t, grid, smem, stream); break;
+      case 28: rc = launch_knn_tc_kp28(pl.packed, t, grid, smem, stream); break;
+      case 40: rc = launch_knn_tc_kp40(pl.packed, t, grid, smem, stream); break;
+      default: rc = launch_knn_tc_kp56(pl.packed, t, grid, smem, stream); break;
     }
     if (rc != DGCN_OK) return rc;
     DGCN_LAUNCH_CHECK();
@@ -210,97 +317,39 @@ static int launch_knn_tc(KnnArgs& a, Workspace& ws, cudaStream_t stream, const f
       debug_certification_add(failed, static_cast<int64_t>(B) * N);
     }
   }
-  if (n_partial) *n_partial = n_cta + TC_FALLBACK_GRID;
   return DGCN_OK;
 }
 
-// Runs the selection (+ fused consumer described by a.epi) on `stream`.
-// n_partial (optional out): number of train-mode statistic rows the chosen path wrote.
-// true when launch_knn will take the tensor-core path for these arguments
-static bool knn_takes_tc(const KnnArgs& a) {
-  const bool train_wide = a.epi.mode == EPI_EDGE && a.epi.norm == DGCN_NORM_BATCH_TRAIN && a.epi.c_out > 128;
-  return !a.exact_fp32 && tc_shape_ok(a.C, a.N, a.K) && a.k <= SEL_LD && !train_wide;
-}
-// the fused prologue can also produce PQ (EdgeConv): channel / output counts it supports
-static bool prologue_pq_ok(const KnnArgs& a, int64_t M) {
-  return knn_takes_tc(a) && M % 128 == 0 && M <= 256 && a.C <= TC_MAX_C;
-}
-
+// Runs the selection (+ fused consumer described by a.epi) on `stream`, by the route of `pl`, in the regions
+// carve_knn took for that plan.
 // pqf (optional): produce the EdgeConv node GEMM inside the tensor-core prologue; the caller must have
 // checked prologue_pq_ok and skipped node_pq_kernel.
-int launch_knn(KnnArgs& a, Workspace& ws, cudaStream_t stream, int64_t* n_partial = nullptr,
-               const ProloguePq* pqf = nullptr) {
-  const int B = a.B, N = a.N, K = a.K;
-  float* sq = ws.take<float>(static_cast<size_t>(B) * N);
-  if (!ws.ok) return DGCN_ERR_WORKSPACE;
-  a.sq = sq;
-  if (knn_takes_tc(a))
-    return launch_knn_tc(a, ws, stream, a.epi.mode == EPI_MR ? a.epi.xt : nullptr, n_partial, pqf);
+static int launch_knn(KnnArgs& a, const KnnPlan& pl, const KnnRegions& r, cudaStream_t stream,
+                      const ProloguePq* pqf = nullptr) {
+  const int B = a.B, N = a.N;
+  a.sq = r.sq;
+  if (pl.route == KNN_TC) return launch_knn_tc(a, pl, r, stream, pqf);
   if (pqf) return DGCN_ERR_BAD_ARG;   // (internal misuse) nobody would produce PQ
-  const bool rows_on_tc = K > 32 && K <= LARGE_K_MAX && dist_rows_tc_ok(a);   // large-K: distance rows on the tensor cores
-  __nv_bfloat16* planes3 = nullptr;
-  if (rows_on_tc) {
-    planes3 = ws.take<__nv_bfloat16>(dist_rows_tc_plane_elems(B, a.C, N));
-    if (!ws.ok) return DGCN_ERR_WORKSPACE;
-    int rc = dist_rows_tc_prepare(a, planes3, stream);      // sq (same FMA chain as sqnorm_kernel) + the bf16 planes
+  if (pl.rows_on_tc) {
+    int rc = dist_rows_tc_prepare(a, r.planes3, stream);      // sq (same FMA chain as sqnorm_kernel) + the bf16 planes
     if (rc != DGCN_OK) return rc;
   } else {
-    sqnorm_kernel<<<dim3(ceil_div(N, 256), B), 256, 0, stream>>>(a.x, a.sb, a.sc, a.C, N, sq);
+    sqnorm_kernel<<<dim3(ceil_div(N, 256), B), 256, 0, stream>>>(a.x, a.sb, a.sc, a.C, N, r.sq);
     DGCN_LAUNCH_CHECK();
   }
-  const dim3 grid(ceil_div(N, TILE), B);
-  if (n_partial) *n_partial = K <= SMALL_K_MAX ? static_cast<int64_t>(grid.x) * grid.y : static_cast<int64_t>(B) * N;
-  if (K <= 32) {
+  if (pl.route == KNN_SMALL) {
     const size_t smem = sizeof(SmallSmem<1>);
     DGCN_ENSURE_SMEM((knn_small_kernel<1>), smem);
     {
       KernelTimer timer(stream, "knn");
-      knn_small_kernel<1><<<grid, NTHREADS, smem, stream>>>(a);
+      knn_small_kernel<1><<<pl.grid, NTHREADS, smem, stream>>>(a);
     }
     DGCN_LAUNCH_CHECK();
     return DGCN_OK;
   }
-  if (K > LARGE_K_MAX) return DGCN_ERR_UNSUPPORTED;
-  const int ldd = (N + 3) / 4 * 4;
-  const int nbmax = static_cast<int>(knn_slab_clouds(B, N));
-  const size_t slab_elems = static_cast<size_t>(nbmax) * N * ldd;
-  float* drows = ws.take<float>(slab_elems);
-  float* drows2 = B > nbmax ? ws.take<float>(slab_elems) : nullptr;   // second slab: distance rows run one slab ahead
-  if (!ws.ok) return DGCN_ERR_WORKSPACE;
-  const int KP = next_pow2(K);
-  const size_t per_warp = static_cast<size_t>(KP) * 8 + static_cast<size_t>(ldd) * 4 + static_cast<size_t>((a.k + 31) / 32 * 32) * 4;   // ldd = N rounded up to 4 keeps every warp's u64 array 16-byte aligned
-  int warps = static_cast<int>((200u << 10) / per_warp);
-  if (warps < 1) return DGCN_ERR_UNSUPPORTED;   // a single row does not fit in shared memory
-  if (warps > 4) warps = 4;
-  const size_t smem = per_warp * warps;
-  DGCN_ENSURE_SMEM((select_rows_kernel), smem);
-  // sampled fast select: bound = sample_rank-th of 128 samples (mean + 2.5 sigma + 2 of the K/N quantile)
-  const double pq = static_cast<double>(K) / N;
-  int sample_rank = static_cast<int>(128.0 * pq + 2.5 * sqrt(128.0 * pq * (1.0 - pq)) + 2.0) + 1;
-  if (sample_rank > 127) sample_rank = 127;
-  // room for every key below the bound (no power of two needed: only the wanted bins get sorted);
-  // k > 64 keeps the full sort and needs the padded power of two
-  // keys below a bound at sample rank r: mean (r+1)/129 N, relative spread ~ 1/sqrt(r+1); leave 3.5 sigma
-  const double wmean = (sample_rank + 1) / 129.0 * N;
-  const int64_t wcap = static_cast<int64_t>(wmean * (1.0 + 3.5 / sqrt(sample_rank + 1.0))) + 32;
-  int cap = static_cast<int>(wcap > K + 64 ? wcap : K + 64);
-  cap = a.k > 64 ? next_pow2(cap > 2 * K ? cap : 2 * K) : (cap + 31) / 32 * 32;
-  if (cap < 128) cap = 128;            // the sorted sample lives in the same array
-  if (cap > 2048) cap = 2048;
-  const bool fast = N >= 512 && cap >= K;
-  const size_t per_warp_f = static_cast<size_t>(cap) * 8 + static_cast<size_t>((a.k + 31) / 32 * 32) * 4 + 2560;   // keys, sel, multi-select tables (hist 256, prefix 260 ints, 256 marks -> 2320 B)
-  int warps_f = static_cast<int>((56u << 10) / per_warp_f);   // <= 56 KB per CTA: four CTAs per SM
-  if (warps_f > 8) warps_f = 8;
-  if (warps_f < 1) warps_f = 1;
-  const size_t smem_f = per_warp_f * warps_f;
-  int* rowlist = nullptr;
-  int* rowlist2 = nullptr;
-  if (fast) {
-    rowlist = ws.take<int>(static_cast<size_t>(nbmax) * N + 64);
-    if (drows2) rowlist2 = ws.take<int>(static_cast<size_t>(nbmax) * N + 64);
-    if (!ws.ok) return DGCN_ERR_WORKSPACE;
-    DGCN_ENSURE_SMEM((select_rows_fast_kernel), smem_f);
-  }
+  const int ldd = pl.ldd, nbmax = pl.nbmax, warps = pl.warps, warps_f = pl.warps_f;
+  DGCN_ENSURE_SMEM((select_rows_kernel), pl.smem);
+  if (pl.fast) DGCN_ENSURE_SMEM((select_rows_fast_kernel), pl.smem_f);
   KernelTimer timer(stream, "knn");
   // Two-chain slab pipeline: even slabs run (distance rows -> sampled select -> exact completion) on the caller's
   // stream, odd slabs on a side stream with their own row buffer and completion list.  The chains overlap freely:
@@ -308,7 +357,7 @@ int launch_knn(KnnArgs& a, Workspace& ws, cudaStream_t stream, int64_t* n_partia
   // most - the partial last wave of one select (4096 rows are 1.15 .. 2.3 waves of its CTAs) is filled by the CTAs
   // of the other chain.  An event forks the side stream from the caller's stream and one joins it back, so the call
   // is still one stream-ordered operation for the caller (and capturable in a CUDA graph).
-  cudaStream_t side = drows2 ? slab_side_stream() : nullptr;
+  cudaStream_t side = pl.two_slabs ? slab_side_stream() : nullptr;
   cudaEvent_t ev_start = nullptr, ev_join = nullptr;
   if (side) {
     if (cudaEventCreateWithFlags(&ev_start, cudaEventDisableTiming) != cudaSuccess ||
@@ -328,27 +377,27 @@ int launch_knn(KnnArgs& a, Workspace& ws, cudaStream_t stream, int64_t* n_partia
     const int nb = (B - b0 < nbmax) ? (B - b0) : nbmax;
     const int buf = side ? (slab & 1) : 0;
     cudaStream_t st = buf ? side : stream;             // a buffer is only ever touched by its own chain: stream order
-    float* drows_s = buf ? drows2 : drows;
-    int* rowlist_s = buf ? rowlist2 : rowlist;
-    if (rows_on_tc) {
-      int rc = dist_rows_tc_launch(a, planes3, b0, nb, drows_s, ldd, st);
+    float* drows_s = r.drows[buf];
+    int* rowlist_s = r.rowlist[buf];
+    if (pl.rows_on_tc) {
+      int rc = dist_rows_tc_launch(a, r.planes3, b0, nb, drows_s, ldd, st);
       if (rc != DGCN_OK) return rc;
     } else {
       dist_rows_kernel<<<dim3(ceil_div(N, TILE), ceil_div(N, TILE), nb), NTHREADS, 0, st>>>(a, b0, drows_s, ldd);
       DGCN_LAUNCH_CHECK();
     }
     const int64_t rows = static_cast<int64_t>(nb) * N;
-    if (fast) {
+    if (pl.fast) {
       DGCN_CUDA_TRY(cudaMemsetAsync(rowlist_s, 0, 256, st));
-      select_rows_fast_kernel<<<static_cast<unsigned>(ceil_div(rows, warps_f)), warps_f * 32, smem_f, st>>>(
-          a, b0, nb, drows_s, ldd, cap, sample_rank, warps_f, rowlist_s, rowlist_s + 64);
+      select_rows_fast_kernel<<<static_cast<unsigned>(ceil_div(rows, warps_f)), warps_f * 32, pl.smem_f, st>>>(
+          a, b0, nb, drows_s, ldd, pl.cap, pl.sample_rank, warps_f, rowlist_s, rowlist_s + 64);
       DGCN_LAUNCH_CHECK();
-      select_rows_kernel<<<2 * device_sm_count(), warps * 32, smem, st>>>(a, b0, nb, drows_s, ldd, KP, ldd, warps, rowlist_s + 64,
-                                                                      rowlist_s);   // grid-stride over the handed-over rows
+      select_rows_kernel<<<pl.select_grid, warps * 32, pl.smem, st>>>(a, b0, nb, drows_s, ldd, pl.KP, ldd, warps,
+                                                                    rowlist_s + 64, rowlist_s);
       DGCN_LAUNCH_CHECK();
     } else {
-      select_rows_kernel<<<static_cast<unsigned>(ceil_div(rows, warps)), warps * 32, smem, st>>>(
-          a, b0, nb, drows_s, ldd, KP, ldd, warps, nullptr, nullptr);
+      select_rows_kernel<<<static_cast<unsigned>(ceil_div(rows, warps)), warps * 32, pl.smem, st>>>(
+          a, b0, nb, drows_s, ldd, pl.KP, ldd, warps, nullptr, nullptr);
       DGCN_LAUNCH_CHECK();
     }
   }
@@ -684,35 +733,41 @@ __global__ void __launch_bounds__(256) graph_gather_kernel(const GatherArgs g) {
   }
 }
 
-// ---- planning -----------------------------------------------------------------------------
-struct ConvPlan {
-  size_t wk, bk, pq, xt, r, out_min, partial, st;   // element counts (floats)
-  int64_t n_partial;
+// ---- convolution workspace ------------------------------------------------------------------
+struct ConvRegions {
+  int64_t n_partial;         // train-mode statistic rows: one per CTA of whatever writes them
+  float* wk;                 // packed weights
+  float* st;                 // BatchNorm (scale, shift)
+  float* partial;            // train mode: [n_partial][2][co] sum / sum of squares of act()
+  float* bk;                 // EdgeConv: packed bias
+  float* pq;                 // EdgeConv: node GEMM (B,N,2co)
+  float* out_min;            // EdgeConv, train mode: min over neighbours of act()
+  float* xt;                 // MRConv: node-major copy of x
+  float* r;                  // MRConv: max_j x_j - x_i
+  KnnRegions knn;            // fused graph: the selection's regions
 };
-static ConvPlan conv_plan(int conv, int64_t B, int64_t ci, int64_t co, int64_t N, int64_t K, bool fused) {
-  ConvPlan p{};
-  p.st = 2 * co;
-  if (conv == DGCN_CONV_EDGE) {
-    p.wk = ci * 2 * co;
-    p.bk = 2 * co;
-    p.pq = B * N * 2 * co;
-    p.out_min = B * co * N;
-    int64_t tiles = fused ? (K <= SMALL_K_MAX ? ceil_div(N, TILE) * B + TC_FALLBACK_GRID : B * N) : ceil_div(N, 32) * B;
-    p.n_partial = tiles;
-    p.partial = tiles * 2 * co;
+
+// The regions of conv_forward in the order it uses them; a / kp: the selection's arguments and plan when the graph is
+// fused, null for a given graph.
+static ConvRegions carve_conv(int conv, int64_t B, int64_t ci, int64_t co, int64_t N, bool train, const KnnArgs* a,
+                              const KnnPlan* kp, Workspace& ws) {
+  ConvRegions r{};
+  const bool edge = conv == DGCN_CONV_EDGE;
+  // the statistics come from the selection's epilogue, graph_gather_kernel or mr_node_kernel
+  r.n_partial = !edge ? ceil_div(N, TILE) * B : kp ? kp->n_partial : ceil_div(N, 32) * B;
+  r.wk = ws.take<float>(2 * ci * co);
+  r.st = ws.take<float>(2 * co);
+  r.partial = train ? ws.take<float>(r.n_partial * 2 * co) : nullptr;
+  if (edge) {
+    r.bk = ws.take<float>(2 * co);
+    r.pq = ws.take<float>(B * N * 2 * co);
+    r.out_min = train ? ws.take<float>(B * co * N) : nullptr;
   } else {
-    p.wk = 2 * ci * co;
-    p.xt = B * N * ci;
-    p.r = B * ci * N;
-    p.n_partial = B * ceil_div(N, TILE);
-    p.partial = p.n_partial * 2 * co;
+    r.xt = ws.take<float>(B * N * ci);
+    r.r = ws.take<float>(B * ci * N);
   }
-  return p;
-}
-static size_t conv_plan_bytes(const ConvPlan& p) {
-  size_t b = 0;
-  for (size_t v : {p.wk, p.bk, p.pq, p.xt, p.r, p.out_min, p.partial, p.st}) b += align_up(v * 4, 256);
-  return b + 256;
+  if (kp) r.knn = carve_knn(*a, *kp, ws);
+  return r;
 }
 
 static int check_conv_args(int conv, const float* x, int64_t B, int64_t ci, int64_t N, const dgcn_basic_conv* p,
@@ -746,13 +801,13 @@ static int conv_forward(int conv, const float* x, int64_t B, int64_t ci, int64_t
     if (!fused || p->norm == DGCN_NORM_BATCH_TRAIN) return DGCN_ERR_UNSUPPORTED;
     if (fus->out_stride_b != 0 && fus->out_stride_b < co * N) return DGCN_ERR_BAD_ARG;
   }
-  const int64_t K = fused ? dil->k * dil->dilation : k;
   const int64_t keep = fused ? dil->k : k;
-  ConvPlan pl = conv_plan(conv, B, ci, co, N, K, fused);
   const bool train = p->norm == DGCN_NORM_BATCH_TRAIN;
+  const bool edge = conv == DGCN_CONV_EDGE;
   const int vec = ((reinterpret_cast<uintptr_t>(x) & 15) == 0 && sb % 4 == 0 && sc % 4 == 0 && N % 4 == 0) ? 1 : 0;
 
   Epilogue e{};
+  e.mode = edge ? EPI_EDGE : EPI_MR;
   e.nbr = nbr_out;
   e.slope = act_slope_of(p);
   e.prelu = p->act == DGCN_ACT_PRELU ? p->prelu_weight : nullptr;
@@ -761,105 +816,79 @@ static int conv_forward(int conv, const float* x, int64_t B, int64_t ci, int64_t
   e.c_out = static_cast<int>(co);
   e.c_in = static_cast<int>(ci);
   e.out_sb = (fus && fus->out_stride_b) ? fus->out_stride_b : co * N;
-  if (fus && fus->residual && conv == DGCN_CONV_EDGE) {   // (MRConv adds it in its node kernel)
+  if (fus && fus->residual && edge) {   // (MRConv adds it in its node kernel)
     e.res = fus->residual; e.res_sb = fus->res_stride_b; e.res_sc = fus->res_stride_c; e.res_scale = fus->res_scale;
   }
-  float* wk = ws.take<float>(pl.wk);
-  float* st = ws.take<float>(pl.st);
-  float* partial = train ? ws.take<float>(pl.partial) : nullptr;
-  if (!ws.ok) return DGCN_ERR_WORKSPACE;
-
-  if (conv == DGCN_CONV_EDGE) {
-    float* bk = ws.take<float>(pl.bk);
-    float* pq = ws.take<float>(pl.pq);
-    float* out_min = train ? ws.take<float>(pl.out_min) : nullptr;
-    if (!ws.ok) return DGCN_ERR_WORKSPACE;
-    const int M = static_cast<int>(2 * co);
-    pack_edge_weights_kernel<<<static_cast<unsigned>(ceil_div(ci * M > M ? ci * M : M, 256)), 256, 0, stream>>>(
-        p->weight, p->bias, static_cast<int>(ci), static_cast<int>(co), wk, bk);
-    DGCN_LAUNCH_CHECK();
-    e.mode = EPI_EDGE;
-    e.pq = pq;
-    e.out = out;
-    e.out_min = out_min;
-    e.partial = partial;
-    KnnArgs a;
-    bool pq_in_prologue = false;
-    if (fused) {
-      int rc = fill_knn_args(a, x, B, ci, N, sb, sc, dil, 0);
-      if (rc != DGCN_OK) return rc;
-      a.epi = e;
-      pq_in_prologue = prologue_pq_ok(a, M);   // the tensor-core prologue computes PQ on its pass over x
-    }
-    if (!pq_in_prologue) {
-      node_pq_kernel<<<dim3(ceil_div(M, TILE), ceil_div(N, TILE), B), NTHREADS, 0, stream>>>(
-          x, sb, sc, static_cast<int>(ci), static_cast<int>(N), vec, wk, bk, M, pq);
-      DGCN_LAUNCH_CHECK();
-    }
-    if (fused) {
-      const ProloguePq pqf{wk, bk, pq, static_cast<int>(M)};
-      int rc = launch_knn(a, ws, stream, &pl.n_partial, pq_in_prologue ? &pqf : nullptr);
-      if (rc != DGCN_OK) return rc;
-    } else {
-      GatherArgs g{e, edge_index, nbr, static_cast<int>(B), static_cast<int>(N), static_cast<int>(k)};
-      graph_gather_kernel<<<dim3(ceil_div(N, 32), B), 256, 0, stream>>>(g);
-      DGCN_LAUNCH_CHECK();
-    }
-    if (train) {
-      int rc = bn_finalize(partial, pl.n_partial, co, static_cast<double>(B) * N * keep, p, sync, st, stream);
-      if (rc != DGCN_OK) return rc;
-      const int64_t total = B * co * N;
-      bn_apply_kernel<<<static_cast<unsigned>(ceil_div(total, 256)), 256, 0, stream>>>(
-          out, out_min, st, static_cast<int>(co), static_cast<int>(N), total);
-      DGCN_LAUNCH_CHECK();
-    }
-    return DGCN_OK;
-  }
-
-  // MRConv: r = max_j x_j - x_i (gather on a node-major copy), then the node update GEMM
-  float* xt = ws.take<float>(pl.xt);
-  float* r = ws.take<float>(pl.r);
-  if (!ws.ok) return DGCN_ERR_WORKSPACE;
-  pack_mr_weights_kernel<<<static_cast<unsigned>(ceil_div(2 * ci * co, 256)), 256, 0, stream>>>(
-      p->weight, static_cast<int>(2 * ci), static_cast<int>(co), wk);
-  DGCN_LAUNCH_CHECK();
-  to_node_major_kernel<<<dim3(ceil_div(N, 32), ceil_div(ci, 32), B), dim3(32, 8), 0, stream>>>(
-      x, sb, sc, static_cast<int>(ci), static_cast<int>(N), xt);
-  DGCN_LAUNCH_CHECK();
-  e.mode = EPI_MR;
-  e.xt = xt;
-  e.r_out = r;
+  KnnArgs a;
+  KnnPlan kp;
   if (fused) {
-    KnnArgs a;
     int rc = fill_knn_args(a, x, B, ci, N, sb, sc, dil, 0);
     if (rc != DGCN_OK) return rc;
     a.epi = e;
-    rc = launch_knn(a, ws, stream);
+    rc = knn_plan(a, device_limits(), kp);
+    if (rc != DGCN_OK) return rc;
+  }
+  const ConvRegions w = carve_conv(conv, B, ci, co, N, train, fused ? &a : nullptr, fused ? &kp : nullptr, ws);
+  if (!ws.ok) return DGCN_ERR_WORKSPACE;
+  bool pq_in_prologue = false;
+
+  if (edge) {
+    const int M = static_cast<int>(2 * co);
+    pack_edge_weights_kernel<<<static_cast<unsigned>(ceil_div(ci * M > M ? ci * M : M, 256)), 256, 0, stream>>>(
+        p->weight, p->bias, static_cast<int>(ci), static_cast<int>(co), w.wk, w.bk);
+    DGCN_LAUNCH_CHECK();
+    e.pq = w.pq;
+    e.out = out;
+    e.out_min = w.out_min;
+    e.partial = w.partial;
+    pq_in_prologue = fused && prologue_pq_ok(kp, M);   // the tensor-core prologue computes PQ on its pass over x
+    if (!pq_in_prologue) {
+      node_pq_kernel<<<dim3(ceil_div(M, TILE), ceil_div(N, TILE), B), NTHREADS, 0, stream>>>(
+          x, sb, sc, static_cast<int>(ci), static_cast<int>(N), vec, w.wk, w.bk, M, w.pq);
+      DGCN_LAUNCH_CHECK();
+    }
+  } else {   // MRConv: r = max_j x_j - x_i (gather on a node-major copy), then the node update GEMM
+    pack_mr_weights_kernel<<<static_cast<unsigned>(ceil_div(2 * ci * co, 256)), 256, 0, stream>>>(
+        p->weight, static_cast<int>(2 * ci), static_cast<int>(co), w.wk);
+    DGCN_LAUNCH_CHECK();
+    to_node_major_kernel<<<dim3(ceil_div(N, 32), ceil_div(ci, 32), B), dim3(32, 8), 0, stream>>>(
+        x, sb, sc, static_cast<int>(ci), static_cast<int>(N), w.xt);
+    DGCN_LAUNCH_CHECK();
+    e.xt = w.xt;
+    e.r_out = w.r;
+  }
+  if (fused) {
+    a.epi = e;
+    const ProloguePq pqf{w.wk, w.bk, w.pq, static_cast<int>(2 * co)};
+    int rc = launch_knn(a, kp, w.knn, stream, pq_in_prologue ? &pqf : nullptr);
     if (rc != DGCN_OK) return rc;
   } else {
     GatherArgs g{e, edge_index, nbr, static_cast<int>(B), static_cast<int>(N), static_cast<int>(k)};
     graph_gather_kernel<<<dim3(ceil_div(N, 32), B), 256, 0, stream>>>(g);
     DGCN_LAUNCH_CHECK();
   }
-  MrNodeArgs m{};
-  m.x = x; m.sb = sb; m.sc = sc; m.r = r; m.ci = static_cast<int>(ci); m.N = static_cast<int>(N); m.vec = vec;
-  m.wk = wk; m.bias = p->bias; m.co = static_cast<int>(co);
-  m.slope = e.slope; m.prelu = e.prelu;
-  m.norm = p->norm; m.bn_w = p->bn_weight; m.bn_b = p->bn_bias; m.bn_m = p->bn_mean; m.bn_v = p->bn_var;
-  m.bn_eps = p->bn_eps;
-  m.out = out; m.partial = partial;
-  m.out_sb = e.out_sb;
-  if (fus && fus->residual) {
-    m.res = fus->residual; m.res_sb = fus->res_stride_b; m.res_sc = fus->res_stride_c; m.res_scale = fus->res_scale;
+  if (!edge) {
+    MrNodeArgs m{};
+    m.x = x; m.sb = sb; m.sc = sc; m.r = w.r; m.ci = static_cast<int>(ci); m.N = static_cast<int>(N); m.vec = vec;
+    m.wk = w.wk; m.bias = p->bias; m.co = static_cast<int>(co);
+    m.slope = e.slope; m.prelu = e.prelu;
+    m.norm = p->norm; m.bn_w = p->bn_weight; m.bn_b = p->bn_bias; m.bn_m = p->bn_mean; m.bn_v = p->bn_var;
+    m.bn_eps = p->bn_eps;
+    m.out = out; m.partial = w.partial;
+    m.out_sb = e.out_sb;
+    if (fus && fus->residual) {
+      m.res = fus->residual; m.res_sb = fus->res_stride_b; m.res_sc = fus->res_stride_c; m.res_scale = fus->res_scale;
+    }
+    mr_node_kernel<<<dim3(ceil_div(N, TILE), ceil_div(co, TILE), B), NTHREADS, 0, stream>>>(m);
+    DGCN_LAUNCH_CHECK();
   }
-  mr_node_kernel<<<dim3(ceil_div(N, TILE), ceil_div(co, TILE), B), NTHREADS, 0, stream>>>(m);
-  DGCN_LAUNCH_CHECK();
-  if (train) {
-    int rc = bn_finalize(partial, pl.n_partial, co, static_cast<double>(B) * N, p, sync, st, stream);
+  if (train) {   // EdgeConv normalises the B*N*keep edge activations, MRConv the B*N node activations
+    int rc = bn_finalize(w.partial, w.n_partial, co, static_cast<double>(B) * N * (edge ? keep : 1), p, sync, w.st,
+                         stream);
     if (rc != DGCN_OK) return rc;
     const int64_t total = B * co * N;
     bn_apply_kernel<<<static_cast<unsigned>(ceil_div(total, 256)), 256, 0, stream>>>(
-        out, nullptr, st, static_cast<int>(co), static_cast<int>(N), total);
+        out, w.out_min, w.st, static_cast<int>(co), static_cast<int>(N), total);
     DGCN_LAUNCH_CHECK();
   }
   return DGCN_OK;
@@ -871,8 +900,12 @@ using namespace dgcn;
 
 extern "C" {
 
+// The workspace queries run the launch's carve in counting mode and report 256 bytes past its last region (512 for
+// the dyn conv, which counts the convolution's regions and the selection's); nothing is placed there.
+
 size_t dgcn_knn_graph_workspace_bytes(int64_t B, int64_t C, int64_t N, int64_t K) {
-  return knn_workspace_bytes(B, C, N, K);
+  return max_over_routes(B, C, N, K, EPI_INDEX, 0,
+                         [](const KnnArgs& a, const KnnPlan& p, Workspace& ws) { carve_knn(a, p, ws); }) + 256;
 }
 
 int dgcn_knn_graph(const float* x, int64_t B, int64_t C, int64_t N, int64_t stride_b, int64_t stride_c,
@@ -884,12 +917,20 @@ int dgcn_knn_graph(const float* x, int64_t B, int64_t C, int64_t N, int64_t stri
   if (!edge_index && !nbr) return DGCN_ERR_BAD_ARG;
   a.epi.edge_index = edge_index;
   a.epi.nbr = nbr;
+  KnnPlan pl;
+  rc = knn_plan(a, device_limits(), pl);
+  if (rc != DGCN_OK) return rc;
   Workspace ws(wsp, ws_bytes);
-  return launch_knn(a, ws, static_cast<cudaStream_t>(stream));
+  const KnnRegions r = carve_knn(a, pl, ws);
+  if (!ws.ok) return DGCN_ERR_WORKSPACE;
+  return launch_knn(a, pl, r, static_cast<cudaStream_t>(stream));
 }
 
 size_t dgcn_graph_conv_workspace_bytes(int32_t conv, int64_t B, int64_t C_in, int64_t C_out, int64_t N, int64_t k) {
-  return conv_plan_bytes(conv_plan(conv, B, C_in, C_out, N, k, false));
+  (void)k;
+  Workspace ws;
+  carve_conv(conv, B, C_in, C_out, N, true, nullptr, nullptr, ws);   // train mode carves the most
+  return ws.off + 256;
 }
 
 int dgcn_graph_conv_forward(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N, int64_t stride_b,
@@ -914,7 +955,10 @@ int dgcn_graph_conv_forward_sync(int32_t conv, const float* x, int64_t B, int64_
 }
 
 size_t dgcn_dyn_conv_workspace_bytes(int32_t conv, int64_t B, int64_t C_in, int64_t C_out, int64_t N, int64_t K) {
-  return conv_plan_bytes(conv_plan(conv, B, C_in, C_out, N, K, true)) + knn_workspace_bytes(B, C_in, N, K);
+  return max_over_routes(B, C_in, N, K, conv == DGCN_CONV_EDGE ? EPI_EDGE : EPI_MR, C_out,
+                         [&](const KnnArgs& a, const KnnPlan& p, Workspace& ws) {
+                           carve_conv(conv, B, C_in, C_out, N, a.epi.norm == DGCN_NORM_BATCH_TRAIN, &a, &p, ws);
+                         }) + 512;
 }
 
 int dgcn_dyn_conv_forward(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N, int64_t stride_b,

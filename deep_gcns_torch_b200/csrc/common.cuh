@@ -152,6 +152,55 @@ __device__ __forceinline__ float warp_max(float v) {
 // 0.2 leakyrelu, learnt prelu weight, 1 identity.
 __device__ __forceinline__ float act_apply(float z, float slope) { return z >= 0.f ? z : z * slope; }
 
+// ---- train-mode BatchNorm statistics ------------------------------------------
+// A channel's batch statistics travel as (count, mean, M2 = sum of squared deviations from the mean), never as
+// (sum a, sum a^2): E[a^2] - E[a]^2 in fp32 loses ~ (mean / std)^2 * 2^-24 of the variance, which a channel with a
+// large mean (un-centred coordinates, a ReLU channel dominated by its bias) turns into percent errors.  A thread
+// sums a - pivot and (a - pivot)^2, pivot = the first value it saw, so its sums are of the channel's spread only;
+// threads and warps merge (count, mean, M2) with Chan's formula in fp32; the partial rows [n_partial][3][C] of a
+// launch are merged the same way in fp64 (bn_merge_kernel).  A constant channel stays exact: every deviation and
+// every mean difference is 0, so the variance is 0 and the mean the constant.
+constexpr int BN_PARTIAL_ROWS = 3;   // a partial row: count, mean, M2 (each [C])
+
+struct BnAcc { float n, pivot, d1, d2; };     // one thread's running sums
+struct BnMoments { float n, mean, m2; };
+
+__device__ __forceinline__ BnAcc bn_acc_zero() { return BnAcc{0.f, 0.f, 0.f, 0.f}; }
+__device__ __forceinline__ void bn_acc_add(BnAcc& s, float a) {
+  s.pivot = s.n == 0.f ? a : s.pivot;
+  const float d = a - s.pivot;
+  s.n += 1.f;
+  s.d1 += d;
+  s.d2 = fmaf(d, d, s.d2);
+}
+__device__ __forceinline__ BnMoments bn_acc_moments(const BnAcc& s) {
+  if (s.n == 0.f) return BnMoments{0.f, 0.f, 0.f};
+  const float m = s.d1 / s.n;
+  return BnMoments{s.n, s.pivot + m, fmaxf(fmaf(-s.d1, m, s.d2), 0.f)};
+}
+// Chan et al.: merge of two disjoint sets; either (or both) may be empty
+__device__ __forceinline__ BnMoments bn_merge(const BnMoments& a, const BnMoments& b) {
+  const float n = a.n + b.n;
+  const float f = n > 0.f ? b.n / n : 0.f;
+  const float delta = b.mean - a.mean;
+  return BnMoments{n, fmaf(delta, f, a.mean), a.m2 + b.m2 + delta * (delta * (a.n * f))};
+}
+__device__ __forceinline__ BnMoments bn_shfl_xor(const BnMoments& m, int o) {
+  return BnMoments{__shfl_xor_sync(0xffffffffu, m.n, o), __shfl_xor_sync(0xffffffffu, m.mean, o),
+                   __shfl_xor_sync(0xffffffffu, m.m2, o)};
+}
+// partial row `row`, channel c of C
+__device__ __forceinline__ void bn_store_partial(float* partial, int64_t row, int C, int c, const BnMoments& m) {
+  float* p = partial + row * BN_PARTIAL_ROWS * C + c;
+  p[0] = m.n;
+  p[C] = m.mean;
+  p[2 * static_cast<int64_t>(C)] = m.m2;
+}
+__device__ __forceinline__ BnMoments bn_load_partial(const float* partial, int64_t row, int C, int c) {
+  const float* p = partial + row * BN_PARTIAL_ROWS * C + c;
+  return BnMoments{p[0], p[C], p[2 * static_cast<int64_t>(C)]};
+}
+
 // ---- 128x128 fp32 tile engine ------------------------------------------------
 // C[r][c] = sum_k A[k][r] * B[k][c] for one 128x128 output tile, A and B both
 // "k-major" (row k contiguous along r / c).  256 threads, 8x8 accumulators per

@@ -147,8 +147,9 @@ __global__ void reduce_partials_kernel(const float* __restrict__ partial, int64_
 
 __global__ void store_count_kernel(double* __restrict__ dst, double count) { *dst = count; }
 
-// Synced BatchNorm statistics (dgcn_bn_sync), forward and backward: sync->moments = [the fixed-order fp64 sums of
-// rows q = 0, 1 of the [np][nq][C] partials | count], then the caller enqueues their cross-rank sum on `stream`.
+// Synced backward sums (dgcn_bn_sync): sync->moments = [the fixed-order fp64 sums of rows q = 0, 1 of the
+// [np][nq][C] partials | count], then the caller enqueues their cross-rank sum on `stream`.  (The forward's
+// statistics partials are (count, mean, M2) rows: bn_merge_kernel, dense_fwd.cu.)
 int bn_sync_moments(const float* partial, int64_t np, int nq, int C, double count, const dgcn_bn_sync* sync,
                     cudaStream_t stream) {
   reduce_partials_kernel<<<dim3(C, 2), 256, 0, stream>>>(partial, np, nq, C, sync->moments);

@@ -307,7 +307,7 @@ static int launch_knn_tc(KnnArgs& a, const KnnPlan& pl, const KnnRegions& r, cud
     }
     if (rc != DGCN_OK) return rc;
     DGCN_LAUNCH_CHECK();
-    float* extra = a.epi.partial ? a.epi.partial + n_cta * 2 * a.epi.c_out : nullptr;
+    float* extra = a.epi.partial ? a.epi.partial + n_cta * BN_PARTIAL_ROWS * a.epi.c_out : nullptr;
     knn_exact_rows_kernel<<<TC_FALLBACK_GRID, 256, 0, stream>>>(a, t.fail_count, t.fail_list, extra);
     DGCN_LAUNCH_CHECK();
     if (debug_certification_on()) {
@@ -535,7 +535,7 @@ __global__ void __launch_bounds__(NTHREADS, 2) mr_node_kernel(const MrNodeArgs g
         t = (g.bn_b ? __ldg(g.bn_b + m) : 0.f) - __ldg(g.bn_m + m) * s;
       }
     }
-    float s1 = 0.f, s2 = 0.f;
+    BnAcc st = bn_acc_zero();
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const int n = n0 + tile_col(tx, j);
@@ -544,34 +544,24 @@ __global__ void __launch_bounds__(NTHREADS, 2) mr_node_kernel(const MrNodeArgs g
         float v = fmaf(s, a, t);
         if (g.res) v = __fadd_rn(v, __fmul_rn(__ldg(g.res + b * g.res_sb + m * g.res_sc + n), g.res_scale));
         g.out[b * g.out_sb + static_cast<int64_t>(m) * g.N + n] = v;
-        s1 += a;
-        s2 += a * a;
+        if (train) bn_acc_add(st, a);
       }
     }
-    if (train) {   // reduce over the 16 tx lanes that share this row (lanes differ in low 4 bits)
+    if (train) {   // merge over the 16 tx lanes that share this row (lanes differ in low 4 bits)
+      BnMoments mo = bn_acc_moments(st);
 #pragma unroll
-      for (int o = 8; o > 0; o >>= 1) {
-        s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-        s2 += __shfl_xor_sync(0xffffffffu, s2, o);
-      }
-      if (tx == 0 && m < g.co) {
-        const int64_t slot = static_cast<int64_t>(b) * gridDim.x + blockIdx.x;
-        g.partial[(slot * 2 + 0) * g.co + m] = s1;
-        g.partial[(slot * 2 + 1) * g.co + m] = s2;
-      }
+      for (int o = 8; o > 0; o >>= 1) mo = bn_merge(mo, bn_shfl_xor(mo, o));
+      if (tx == 0 && m < g.co) bn_store_partial(g.partial, static_cast<int64_t>(b) * gridDim.x + blockIdx.x, g.co, m, mo);
     }
   }
 }
 
-// Channel c's (sum a, sum a^2) over `count` positions -> (scale, shift) and the batch mean / biased
-// variance the host needs for the running-stat update (torch BatchNorm2d training semantics: normalise
-// with biased variance).
-__device__ __forceinline__ void bn_finalize_channel(double s1, double s2, double count, int C, int c,
+// Channel c's batch mean and biased variance -> (scale, shift), and both for the host's running-stat update
+// (torch BatchNorm2d training semantics: normalise with biased variance).
+__device__ __forceinline__ void bn_finalize_channel(double mean, double var, int C, int c,
                                                     const float* __restrict__ bn_w, const float* __restrict__ bn_b,
                                                     float eps, float* __restrict__ st, float* __restrict__ mean_out,
                                                     float* __restrict__ var_out) {
-  double mean = s1 / count;
-  double var = s2 / count - mean * mean;
   if (var < 0.0) var = 0.0;
   float inv = 1.0f / sqrtf(static_cast<float>(var) + eps);
   float s = (bn_w ? bn_w[c] : 1.f) * inv;
@@ -581,54 +571,82 @@ __device__ __forceinline__ void bn_finalize_channel(double s1, double s2, double
   if (var_out) var_out[c] = static_cast<float>(var);
 }
 
-// Batch statistics from partial sums (fixed order, fp64), one CTA per channel.
-__global__ void bn_finalize_kernel(const float* __restrict__ partial, int64_t np, int C, double count,
-                                   const float* __restrict__ bn_w, const float* __restrict__ bn_b, float eps,
-                                   float* __restrict__ st, float* __restrict__ mean_out,
-                                   float* __restrict__ var_out) {
-  __shared__ double r1[256], r2[256];
+// fp64 Chan merge of two disjoint sets' (count, mean, M2); either may be empty
+__device__ __forceinline__ void bn_merge64(double& n, double& mean, double& m2, double nb, double meanb, double m2b) {
+  const double t = n + nb;
+  const double f = t > 0.0 ? nb / t : 0.0;
+  const double delta = meanb - mean;
+  m2 += m2b + delta * (delta * (n * f));
+  mean += delta * f;
+  n = t;
+}
+
+// Batch statistics from the [np][3][C] partial rows (common.cuh), merged in fp64 in a fixed order, one CTA per
+// channel.  Local statistics: (scale, shift), batch mean and variance.  Synced (moments != null): this rank's
+// [sum a | sum a^2 | count] of the dgcn_bn_sync ABI, formed in fp64 from the merged (count, mean, M2).
+__global__ void bn_merge_kernel(const float* __restrict__ partial, int64_t np, int C, double count,
+                                const float* __restrict__ bn_w, const float* __restrict__ bn_b, float eps,
+                                float* __restrict__ st, float* __restrict__ mean_out, float* __restrict__ var_out,
+                                double* __restrict__ moments) {
+  __shared__ double rn[256], rm[256], r2[256];
   const int c = blockIdx.x;
-  double a1 = 0.0, a2 = 0.0;
+  double n = 0.0, mean = 0.0, m2 = 0.0;
   for (int64_t i = threadIdx.x; i < np; i += blockDim.x) {
-    a1 += static_cast<double>(partial[(i * 2 + 0) * C + c]);
-    a2 += static_cast<double>(partial[(i * 2 + 1) * C + c]);
+    const BnMoments p = bn_load_partial(partial, i, C, c);
+    bn_merge64(n, mean, m2, p.n, p.mean, p.m2);
   }
-  r1[threadIdx.x] = a1;
-  r2[threadIdx.x] = a2;
+  rn[threadIdx.x] = n;
+  rm[threadIdx.x] = mean;
+  r2[threadIdx.x] = m2;
   __syncthreads();
   for (int o = blockDim.x >> 1; o > 0; o >>= 1) {
     if (threadIdx.x < o) {
-      r1[threadIdx.x] += r1[threadIdx.x + o];
-      r2[threadIdx.x] += r2[threadIdx.x + o];
+      n = rn[threadIdx.x];
+      mean = rm[threadIdx.x];
+      m2 = r2[threadIdx.x];
+      bn_merge64(n, mean, m2, rn[threadIdx.x + o], rm[threadIdx.x + o], r2[threadIdx.x + o]);
+      rn[threadIdx.x] = n;
+      rm[threadIdx.x] = mean;
+      r2[threadIdx.x] = m2;
     }
     __syncthreads();
   }
-  if (threadIdx.x == 0) bn_finalize_channel(r1[0], r2[0], count, C, c, bn_w, bn_b, eps, st, mean_out, var_out);
+  if (threadIdx.x != 0) return;
+  n = rn[0];
+  mean = rm[0];
+  m2 = r2[0];
+  if (moments) {
+    const double s1 = n * mean;
+    moments[c] = s1;
+    moments[C + c] = m2 + s1 * mean;   // bn_finalize_moments_kernel subtracts the same product: M2 comes back exact
+    if (c == 0) moments[2 * C] = count;
+    return;
+  }
+  bn_finalize_channel(mean, n > 0.0 ? m2 / n : 0.0, C, c, bn_w, bn_b, eps, st, mean_out, var_out);
 }
 // Synced statistics (dgcn_bn_sync): the same finalisation from the cross-rank moments [sum a | sum a^2 | count],
-// the count read on the device.
+// the count read on the device.  After the all-reduce the fp64 cancellation costs ~ (mean / std)^2 * 2^-53.
 __global__ void bn_finalize_moments_kernel(const double* __restrict__ moments, int C, const float* __restrict__ bn_w,
                                            const float* __restrict__ bn_b, float eps, float* __restrict__ st,
                                            float* __restrict__ mean_out, float* __restrict__ var_out) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c < C) bn_finalize_channel(moments[c], moments[C + c], moments[2 * C], C, c, bn_w, bn_b, eps, st, mean_out, var_out);
+  if (c >= C) return;
+  const double count = moments[2 * C], s1 = moments[c];
+  const double mean = s1 / count;
+  bn_finalize_channel(mean, (moments[C + c] - s1 * mean) / count, C, c, bn_w, bn_b, eps, st, mean_out, var_out);
 }
-int bn_sync_moments(const float* partial, int64_t np, int nq, int C, double count, const dgcn_bn_sync* sync,
-                    cudaStream_t stream);   // dense_bwd.cu
 
 // Train mode: (scale, shift) into st from the partial rows of `count` positions; with sync, from the
 // statistics of every rank.
 static int bn_finalize(const float* partial, int64_t np, int64_t co, double count, const dgcn_basic_conv* p,
                        const dgcn_bn_sync* sync, float* st, cudaStream_t stream) {
   const int C = static_cast<int>(co);
-  if (!sync) {
-    bn_finalize_kernel<<<static_cast<unsigned>(co), 256, 0, stream>>>(partial, np, C, count, p->bn_weight, p->bn_bias,
-                                                                    p->bn_eps, st, p->batch_mean_out, p->batch_var_out);
-    DGCN_LAUNCH_CHECK();
-    return DGCN_OK;
-  }
-  int rc = bn_sync_moments(partial, np, 2, C, count, sync, stream);
-  if (rc != DGCN_OK) return rc;
+  bn_merge_kernel<<<static_cast<unsigned>(co), 256, 0, stream>>>(partial, np, C, count, p->bn_weight, p->bn_bias,
+                                                                 p->bn_eps, st, p->batch_mean_out, p->batch_var_out,
+                                                                 sync ? sync->moments : nullptr);
+  DGCN_LAUNCH_CHECK();
+  if (!sync) return DGCN_OK;
+  if (sync->reduce(sync->user) != 0) return DGCN_ERR_REDUCE;
   bn_finalize_moments_kernel<<<static_cast<unsigned>(ceil_div(co, 128)), 128, 0, stream>>>(
       sync->moments, C, p->bn_weight, p->bn_bias, p->bn_eps, st, p->batch_mean_out, p->batch_var_out);
   DGCN_LAUNCH_CHECK();
@@ -656,7 +674,7 @@ struct GatherArgs {
 __global__ void __launch_bounds__(256) graph_gather_kernel(const GatherArgs g) {
   __shared__ float smax[32][33];
   __shared__ float smin[32][33];
-  __shared__ float red[8][2][32];
+  __shared__ BnMoments red[8][32];
   const Epilogue& e = g.e;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int b = blockIdx.y, i0 = blockIdx.x * 32;
@@ -669,7 +687,8 @@ __global__ void __launch_bounds__(256) graph_gather_kernel(const GatherArgs g) {
   const int64_t plane = static_cast<int64_t>(g.B) * N * k;
   for (int c0 = 0; c0 < nch; c0 += 32) {
     const int c = c0 + lane;
-    float s1 = 0.f, s2 = 0.f, bs = 1.f, bt = 0.f;
+    float bs = 1.f, bt = 0.f;
+    BnAcc st = bn_acc_zero();
     if (edge) bn_affine(e, c, bs, bt);
     for (int u = 0; u < 4; ++u) {
       const int il = warp * 4 + u, i = i0 + il;
@@ -692,8 +711,7 @@ __global__ void __launch_bounds__(256) graph_gather_kernel(const GatherArgs g) {
           if (edge) {
             const int ld = 2 * e.c_out;
             a = act_apply(__ldg(e.pq + (node0 + ic) * ld + c) + __ldg(e.pq + (node0 + j) * ld + e.c_out + c), slope);
-            s1 += a;
-            s2 += a * a;
+            if (train) bn_acc_add(st, a);
           } else {
             a = __ldg(e.xt + (node0 + j) * e.c_in + c) - __ldg(e.xt + (node0 + ic) * e.c_in + c);
           }
@@ -708,10 +726,7 @@ __global__ void __launch_bounds__(256) graph_gather_kernel(const GatherArgs g) {
         smax[lane][il] = bs >= 0.f ? fmaf(bs, vmax, bt) : fmaf(bs, vmin, bt);
       }
     }
-    if (train) {
-      red[warp][0][lane] = s1;
-      red[warp][1][lane] = s2;
-    }
+    if (train) red[warp][lane] = bn_acc_moments(st);
     __syncthreads();
     float* dst = edge ? e.out : e.r_out;
     for (int t = tid; t < 32 * 32; t += 256) {
@@ -722,12 +737,11 @@ __global__ void __launch_bounds__(256) graph_gather_kernel(const GatherArgs g) {
         if (train) e.out_min[o] = smin[cc][il];
       }
     }
-    if (train && tid < 64) {
-      const int which = tid >> 5, cc = tid & 31;
-      float s = 0.f;
-      for (int w = 0; w < 8; ++w) s += red[w][which][cc];
+    if (train && tid < 32) {
+      BnMoments m = red[0][tid];
+      for (int w = 1; w < 8; ++w) m = bn_merge(m, red[w][tid]);
       const int64_t cta = static_cast<int64_t>(blockIdx.y) * gridDim.x + blockIdx.x;
-      if (c0 + cc < nch) e.partial[(cta * 2 + which) * nch + c0 + cc] = s;
+      if (c0 + tid < nch) bn_store_partial(e.partial, cta, nch, c0 + tid, m);
     }
     __syncthreads();
   }
@@ -738,7 +752,7 @@ struct ConvRegions {
   int64_t n_partial;         // train-mode statistic rows: one per CTA of whatever writes them
   float* wk;                 // packed weights
   float* st;                 // BatchNorm (scale, shift)
-  float* partial;            // train mode: [n_partial][2][co] sum / sum of squares of act()
+  float* partial;            // train mode: [n_partial][3][co] statistics of act() (common.cuh, BnMoments)
   float* bk;                 // EdgeConv: packed bias
   float* pq;                 // EdgeConv: node GEMM (B,N,2co)
   float* out_min;            // EdgeConv, train mode: min over neighbours of act()
@@ -757,7 +771,7 @@ static ConvRegions carve_conv(int conv, int64_t B, int64_t ci, int64_t co, int64
   r.n_partial = !edge ? ceil_div(N, TILE) * B : kp ? kp->n_partial : ceil_div(N, 32) * B;
   r.wk = ws.take<float>(2 * ci * co);
   r.st = ws.take<float>(2 * co);
-  r.partial = train ? ws.take<float>(r.n_partial * 2 * co) : nullptr;
+  r.partial = train ? ws.take<float>(r.n_partial * BN_PARTIAL_ROWS * co) : nullptr;
   if (edge) {
     r.bk = ws.take<float>(2 * co);
     r.pq = ws.take<float>(B * N * 2 * co);

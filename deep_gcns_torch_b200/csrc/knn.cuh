@@ -37,7 +37,7 @@ struct Epilogue {
   const float* bn_w; const float* bn_b; const float* bn_m; const float* bn_v; float bn_eps;
   float* out;            // (B,c_out,N): final value, or max_l act() in train mode
   float* out_min;        // train mode: min_l act()
-  float* partial;        // train mode: [n_cta][2][c_out] sum / sum of squares of act()
+  float* partial;        // train mode: [n_cta][3][c_out] statistics of act() (common.cuh, BnMoments)
   // EPI_MR: xt (B,N,c_in) node-major copy of x ; r_out (B,c_in,N) = max_l x_j - x_i
   const float* xt;
   int c_in;
@@ -88,11 +88,10 @@ __global__ void sqnorm_kernel(const float* __restrict__ x, int64_t sb, int64_t s
 // ---- per-query consumers -------------------------------------------------------
 // One warp, one query (cloud b, point q, already-selected neighbour ids sel[0..k)).
 // Lane owns channel c (may be >= channel count: then it idles).  Returns max / min
-// over neighbours of act(P_q + Q_j) (EDGE) or of x_j (MR, min unused), plus the
-// sum and sum of squares of act() for batch statistics.
+// over neighbours of act(P_q + Q_j) (EDGE) or of x_j (MR, min unused); in train mode
+// act() also goes into the batch statistics st.
 __device__ __forceinline__ void edge_query(const Epilogue& e, int64_t node0, int q, const int* sel,
-                                           int k, int c, float slope, float& vmax, float& vmin,
-                                           float& s1, float& s2) {
+                                           int k, int c, float slope, float& vmax, float& vmin, BnAcc& st) {
   vmax = -INFINITY;
   vmin = INFINITY;
   if (c >= e.c_out) return;
@@ -100,7 +99,8 @@ __device__ __forceinline__ void edge_query(const Epilogue& e, int64_t node0, int
   const float p = __ldg(e.pq + (node0 + q) * ld + c);
   const float* qbase = e.pq + node0 * ld + e.c_out + c;
   int l = 0;
-  if (e.norm != DGCN_NORM_BATCH_TRAIN && slope >= 0.f) {
+  const bool train = e.norm == DGCN_NORM_BATCH_TRAIN;
+  if (!train && slope >= 0.f) {
     // no statistics needed and act is non-decreasing, like the rounded p + q: max / min commute with
     // them bit for bit, so reduce the raw gathered values and activate once
     float rmax = -INFINITY, rmin = INFINITY;
@@ -133,8 +133,12 @@ __device__ __forceinline__ void edge_query(const Epilogue& e, int64_t node0, int
       float a2 = act_apply(p + v[u + 2], slope), a3 = act_apply(p + v[u + 3], slope);
       vmax = fmaxf(fmaxf(vmax, a0), fmaxf(a1, fmaxf(a2, a3)));
       vmin = fminf(fminf(vmin, a0), fminf(a1, fminf(a2, a3)));
-      s1 += (a0 + a1) + (a2 + a3);
-      s2 += (a0 * a0 + a1 * a1) + (a2 * a2 + a3 * a3);
+      if (train) {
+        bn_acc_add(st, a0);
+        bn_acc_add(st, a1);
+        bn_acc_add(st, a2);
+        bn_acc_add(st, a3);
+      }
     }
   }
   for (; l + 4 <= k; l += 4) {
@@ -146,15 +150,18 @@ __device__ __forceinline__ void edge_query(const Epilogue& e, int64_t node0, int
     float a2 = act_apply(p + v2, slope), a3 = act_apply(p + v3, slope);
     vmax = fmaxf(fmaxf(vmax, a0), fmaxf(a1, fmaxf(a2, a3)));
     vmin = fminf(fminf(vmin, a0), fminf(a1, fminf(a2, a3)));
-    s1 += (a0 + a1) + (a2 + a3);
-    s2 += (a0 * a0 + a1 * a1) + (a2 * a2 + a3 * a3);
+    if (train) {
+      bn_acc_add(st, a0);
+      bn_acc_add(st, a1);
+      bn_acc_add(st, a2);
+      bn_acc_add(st, a3);
+    }
   }
   for (; l < k; ++l) {
     float a0 = act_apply(p + __ldg(qbase + static_cast<int64_t>(sel[l]) * ld), slope);
     vmax = fmaxf(vmax, a0);
     vmin = fminf(vmin, a0);
-    s1 += a0;
-    s2 += a0 * a0;
+    if (train) bn_acc_add(st, a0);
   }
 }
 
@@ -228,13 +235,14 @@ __device__ __forceinline__ void cta_epilogue(const KnnArgs& a, int b, int q0, co
   __syncthreads();
   if (e.mode == EPI_INDEX) return;
 
-  float* red = stage_min + 32 * STAGE_LD;                    // [NW][2][32] stat partials
+  BnMoments* red = reinterpret_cast<BnMoments*>(stage_min + 32 * STAGE_LD);   // [NW][32] stat partials
   const bool train = (e.mode == EPI_EDGE && e.norm == DGCN_NORM_BATCH_TRAIN);
   const int nch = (e.mode == EPI_EDGE) ? e.c_out : e.c_in;
   const float slope = (e.mode == EPI_EDGE) ? epi_slope(e) : 0.f;
   for (int c0 = 0; c0 < nch; c0 += 32) {
     const int c = c0 + lane;
-    float s1 = 0.f, s2 = 0.f, bs = 1.f, bt = 0.f;
+    float bs = 1.f, bt = 0.f;
+    BnAcc st = bn_acc_zero();
     if (e.mode == EPI_EDGE) bn_affine(e, c, bs, bt);
     for (int qq = 0; qq < QPW; ++qq) {
       const int ql = warp * QPW + qq;
@@ -242,7 +250,7 @@ __device__ __forceinline__ void cta_epilogue(const KnnArgs& a, int b, int q0, co
       if (qg >= N || (ok != nullptr && !ok[ql])) continue;
       if (e.mode == EPI_EDGE) {
         float vmax, vmin;
-        edge_query(e, node0, qg, &sel[ql * sel_ld], k, c, slope, vmax, vmin, s1, s2);
+        edge_query(e, node0, qg, &sel[ql * sel_ld], k, c, slope, vmax, vmin, st);
         if (train) {
           stage_max[lane * STAGE_LD + ql] = vmax;
           stage_min[lane * STAGE_LD + ql] = vmin;
@@ -253,10 +261,7 @@ __device__ __forceinline__ void cta_epilogue(const KnnArgs& a, int b, int q0, co
         stage_max[lane * STAGE_LD + ql] = mr_query(e, node0, qg, &sel[ql * sel_ld], k, c);
       }
     }
-    if (train) {
-      red[(warp * 2 + 0) * 32 + lane] = s1;
-      red[(warp * 2 + 1) * 32 + lane] = s2;
-    }
+    if (train) red[warp * 32 + lane] = bn_acc_moments(st);
     __syncthreads();
     float* dst = (e.mode == EPI_EDGE) ? e.out : e.r_out;
     const int64_t dst_sb = (e.mode == EPI_EDGE) ? e.out_sb : static_cast<int64_t>(nch) * N;
@@ -270,11 +275,10 @@ __device__ __forceinline__ void cta_epilogue(const KnnArgs& a, int b, int q0, co
         if (train) e.out_min[o] = stage_min[cc * STAGE_LD + ql];
       }
     }
-    if (train && tid < 64) {
-      const int which = tid >> 5, cc = tid & 31;
-      float s = 0.f;
-      for (int w = 0; w < NW; ++w) s += red[(w * 2 + which) * 32 + cc];
-      if (c0 + cc < nch) e.partial[(static_cast<int64_t>(cta) * 2 + which) * nch + c0 + cc] = s;
+    if (train && tid < 32) {
+      BnMoments m = red[tid];
+      for (int w = 1; w < NW; ++w) m = bn_merge(m, red[w * 32 + tid]);
+      if (c0 + tid < nch) bn_store_partial(e.partial, cta, nch, c0 + tid, m);
     }
     __syncthreads();
   }
@@ -286,7 +290,7 @@ __device__ __forceinline__ void cta_epilogue(const KnnArgs& a, int b, int q0, co
 // c_in for MRConv) and N % 8 == 0: a group of G = nch/4 lanes owns one query and reads every selected
 // row as ONE float4 per lane, up to ten rows in flight, so a warp keeps 32 x 10 x 16 B outstanding
 // instead of 8 x 128 B.  A group walks eight consecutive queries and then stores its four channels as
-// full 32-byte sectors; no shared-memory staging.  sel: int [TILE][sel_ld]; red: float [NW][2][nch]
+// full 32-byte sectors; no shared-memory staging.  sel: int [TILE][sel_ld]; red: float [NW][3][nch]
 // (train statistics only).  Each warp only touches the sel rows of its own queries.
 __host__ __device__ __forceinline__ bool epilogue_wide_ok(const KnnArgs& a) {
   const Epilogue& e = a.epi;
@@ -343,7 +347,7 @@ __device__ __forceinline__ void cta_epilogue_wide(const KnnArgs& a, int b, int q
 #pragma unroll
     for (int i = 0; i < 4; ++i) bn_affine(e, 4 * g + i, bs[i], bt[i]);
   }
-  float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
+  BnAcc st[4] = {};
   float* dst = edge ? e.out : e.r_out;
   // eval with a non-decreasing activation (or MRConv's plain max): reduce the raw gathered values
   const bool mono = !TRAIN && (!edge || slope >= 0.f);
@@ -393,10 +397,7 @@ __device__ __forceinline__ void cta_epilogue_wide(const KnnArgs& a, int b, int q
                   const float av = act_apply(pp[c] + w[c], slope);
                   vmax[c] = fmaxf(vmax[c], av);
                   vmin[c] = fminf(vmin[c], av);
-                  if (TRAIN) {
-                    s1[c] += av;
-                    s2[c] = fmaf(av, av, s2[c]);
-                  }
+                  if (TRAIN) bn_acc_add(st[c], av);
                 }
               }
             }
@@ -453,24 +454,18 @@ __device__ __forceinline__ void cta_epilogue_wide(const KnnArgs& a, int b, int q
     }
   }
   if (TRAIN) {
-    // fixed-order reduction: slots of a warp (xor shuffles), then the NW warps in order
+    // fixed-order merge: slots of a warp (xor shuffles), then the NW warps in order
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
-      for (int o = G; o < 32; o <<= 1) {
-        s1[c] += __shfl_xor_sync(0xffffffffu, s1[c], o);
-        s2[c] += __shfl_xor_sync(0xffffffffu, s2[c], o);
-      }
-      if (slot == 0) {
-        red[(warp * 2 + 0) * nch + 4 * g + c] = s1[c];
-        red[(warp * 2 + 1) * nch + 4 * g + c] = s2[c];
-      }
+      BnMoments m = bn_acc_moments(st[c]);
+      for (int o = G; o < 32; o <<= 1) m = bn_merge(m, bn_shfl_xor(m, o));
+      if (slot == 0) bn_store_partial(red, warp, nch, 4 * g + c, m);
     }
     __syncthreads();
-    for (int i = tid; i < 2 * nch; i += NW * 32) {
-      const int which = i / nch, c = i - which * nch;
-      float s = 0.f;
-      for (int w = 0; w < NW; ++w) s += red[(w * 2 + which) * nch + c];
-      e.partial[(static_cast<int64_t>(cta) * 2 + which) * nch + c] = s;
+    for (int c = tid; c < nch; c += NW * 32) {
+      BnMoments m = bn_load_partial(red, 0, nch, c);
+      for (int w = 1; w < NW; ++w) m = bn_merge(m, bn_load_partial(red, w, nch, c));
+      bn_store_partial(e.partial, cta, nch, c, m);
     }
   }
 }
@@ -699,18 +694,17 @@ __device__ __forceinline__ void row_consume(const KnnArgs& a, int b, int q, cons
     const bool train = e.norm == DGCN_NORM_BATCH_TRAIN;
     for (int c0 = 0; c0 < e.c_out; c0 += 32) {
       const int c = c0 + lane;
-      float vmax, vmin, s1 = 0.f, s2 = 0.f, bs, bt;
+      float vmax, vmin, bs, bt;
+      BnAcc st = bn_acc_zero();
       bn_affine(e, c, bs, bt);
-      edge_query(e, node0, q, sel, k, c, slope, vmax, vmin, s1, s2);
+      edge_query(e, node0, q, sel, k, c, slope, vmax, vmin, st);
       if (c < e.c_out) {
         int64_t o = (static_cast<int64_t>(b) * e.c_out + c) * N + q;
         const int64_t oo = b * e.out_sb + static_cast<int64_t>(c) * N + q;
         if (train) {
           e.out[oo] = vmax;
           e.out_min[o] = vmin;
-          // one partial slot per query row: [row][2][c_out]
-          e.partial[(static_cast<int64_t>(node0 + q) * 2 + 0) * e.c_out + c] = s1;
-          e.partial[(static_cast<int64_t>(node0 + q) * 2 + 1) * e.c_out + c] = s2;
+          bn_store_partial(e.partial, node0 + q, e.c_out, c, bn_acc_moments(st));   // one partial row per query
         } else {
           e.out[oo] = epi_res(e, b, c, q, bs >= 0.f ? fmaf(bs, vmax, bt) : fmaf(bs, vmin, bt));
         }

@@ -416,8 +416,8 @@ __host__ __device__ inline int tc_sel_ld(int k) { return k | 1; }
 __host__ __device__ inline size_t tc_work_bytes(int KP, int k, bool wide, int nch) {
   size_t after = static_cast<size_t>(KP) * TILE * 8 + static_cast<size_t>(TILE) * tc_sel_ld(k) * 4;
   after = (after + 15) & ~static_cast<size_t>(15);
-  if (wide) after += static_cast<size_t>(TC_THREADS / 32) * 2 * nch * 4;             // red
-  else after += 2 * static_cast<size_t>(32) * STAGE_LD * 4 + 2 * (TC_THREADS / 32) * 32 * 4 + 256;   // stage_max, stage_min, red
+  if (wide) after += static_cast<size_t>(TC_THREADS / 32) * BN_PARTIAL_ROWS * nch * 4;             // red
+  else after += 2 * static_cast<size_t>(32) * STAGE_LD * 4 + BN_PARTIAL_ROWS * (TC_THREADS / 32) * 32 * 4 + 256;   // stage_max, stage_min, red
   const size_t stream = 2 * static_cast<size_t>(TC_STAGE_BYTES) + 2 * TC_XBLOCK_BYTES;
   const size_t w = after > stream ? after : stream;
   return (w + 1023) & ~static_cast<size_t>(1023);
@@ -829,7 +829,9 @@ __global__ void __launch_bounds__(256) knn_exact_rows_kernel(const KnnArgs a, co
   const int total = *fail_count;
   const Epilogue& e = a.epi;
   const int N = a.N, C = a.C, k = a.k;
-  float s1acc[4] = {0.f, 0.f, 0.f, 0.f}, s2acc[4] = {0.f, 0.f, 0.f, 0.f};   // c_out <= 128 covered per lane
+  BnAcc stacc[4];                          // c_out <= 128 covered per lane
+#pragma unroll
+  for (int u = 0; u < 4; ++u) stacc[u] = bn_acc_zero();
   for (int f = blockIdx.x; f < total; f += gridDim.x) {
     const int code = fail_list[f];
     const int b = code / N, q = code % N;
@@ -894,19 +896,24 @@ __global__ void __launch_bounds__(256) knn_exact_rows_kernel(const KnnArgs a, co
       const bool train = e.norm == DGCN_NORM_BATCH_TRAIN;
       for (int c0 = 0, u = 0; c0 < e.c_out; c0 += 32, ++u) {
         const int c = c0 + lane;
-        float vmax, vmin, s1 = 0.f, s2 = 0.f, bs, bt;
+        float vmax, vmin, bs, bt;
         bn_affine(e, c, bs, bt);
-        edge_query(e, node0, q, sel, k, c, slope, vmax, vmin, s1, s2);
+        // the lane's running statistics of channel c accumulate across the queries of this CTA (selected by
+        // compile-time indices, so that stacc stays in registers)
+        BnAcc st = bn_acc_zero();
+#pragma unroll
+        for (int v = 0; v < 4; ++v)
+          if (v == u) st = stacc[v];
+        edge_query(e, node0, q, sel, k, c, slope, vmax, vmin, st);
+#pragma unroll
+        for (int v = 0; v < 4; ++v)
+          if (v == u) stacc[v] = st;
         if (c < e.c_out) {
           const int64_t o = (static_cast<int64_t>(b) * e.c_out + c) * N + q;
           const int64_t oo = b * e.out_sb + static_cast<int64_t>(c) * N + q;
           if (train) {
             e.out[oo] = vmax;
             e.out_min[o] = vmin;
-            if (u < 4) {
-              s1acc[u] += s1;
-              s2acc[u] += s2;
-            }
           } else {
             e.out[oo] = epi_res(e, b, c, q, bs >= 0.f ? fmaf(bs, vmax, bt) : fmaf(bs, vmin, bt));
           }
@@ -924,12 +931,10 @@ __global__ void __launch_bounds__(256) knn_exact_rows_kernel(const KnnArgs a, co
   // train-mode statistics of the queries completed here: one extra partial row per CTA (warp 0 holds them)
   if (warp == 0 && e.mode == EPI_EDGE && e.norm == DGCN_NORM_BATCH_TRAIN && partial_extra) {
     const int64_t rowi = blockIdx.x;
+#pragma unroll
     for (int u = 0; u < 4; ++u) {
       const int c = u * 32 + lane;
-      if (c < e.c_out) {
-        partial_extra[(rowi * 2 + 0) * e.c_out + c] = s1acc[u];
-        partial_extra[(rowi * 2 + 1) * e.c_out + c] = s2acc[u];
-      }
+      if (c < e.c_out) bn_store_partial(partial_extra, rowi, e.c_out, c, bn_acc_moments(stacc[u]));
     }
   }
 }

@@ -81,14 +81,15 @@ __global__ void __launch_bounds__(256) edge_bwd_kernel(const EdgeBwdArgs g) {
       const int i = i0 + warp * 4 + u;
       if (i >= N || c >= co) continue;
       const float go = __ldg(g.gout + (static_cast<int64_t>(b) * co + c) * N + i);
-      // arg-max edge of y = s*a + t: first max of a when s >= 0, first min otherwise
+      // arg-max edge of y = s*a + t, the first one on a tie as torch.max: first max of a when s > 0, first min when
+      // s < 0, edge 0 when s == 0 (every y equals t)
       float best = 0.f;
       int lbest = 0;
       for (int l = 0; l < k; ++l) {
         int j, ic;
         edge_of(g, node0, i, l, j, ic);
         const float a = act_apply(__ldg(g.pq + (node0 + ic) * ld + c) + __ldg(g.pq + (node0 + j) * ld + co + c), slope);
-        const bool better = (l == 0) || (s >= 0.f ? a > best : a < best);
+        const bool better = (l == 0) || (s > 0.f ? a > best : s < 0.f && a < best);
         if (better) {
           best = a;
           lbest = l;
@@ -107,7 +108,7 @@ __global__ void __launch_bounds__(256) edge_bwd_kernel(const EdgeBwdArgs g) {
           const float ge = (l == lbest) ? go : 0.f;
           float da = s * ge;
           if (train) da = s * (ge - dbeta_n - (a - mean) * inv * dgamma_n);
-          const float dz = z >= 0.f ? da : da * slope;
+          const float dz = z > 0.f ? da : da * slope;     // act'(0) = slope, as torch (relu'(0) = 0)
           if (z < 0.f) acc_sl += z * da;
           atomicAdd(g.dpq + (static_cast<int64_t>(b) * ld + c) * N + ic, dz);
           atomicAdd(g.dpq + (static_cast<int64_t>(b) * ld + co + c) * N + j, dz);
@@ -361,7 +362,7 @@ __global__ void __launch_bounds__(256) mr_bn_bwd_kernel(const MrBnArgs g) {
       float da = s * go;
       if (train) da = s * (go - dbeta_n - ahat * dgamma_n);
       if (z < 0.f) a2 = z * da;
-      g.z[o] = z >= 0.f ? da : da * slope;
+      g.z[o] = z > 0.f ? da : da * slope;             // act'(0) = slope, as torch (relu'(0) = 0)
     }
   }
   red[0][threadIdx.x] = a0;

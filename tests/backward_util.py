@@ -51,8 +51,10 @@ def _kink(z, act):
 def edge_tie_mask(x, edge_index, gconv_nn, act, norm, training):
     """(B,Co,N,1) bool: EdgeConv entries whose max an fp32 kernel may route to a different edge than fp64.
 
-    The max over the edges of y = s*act(z) + t picks the edge of largest act(z) when s >= 0 and of smallest
-    when s < 0.  The kernel ranks act(z) with the sign of s in every mode (edge_bwd_kernel), and its fp32
+    The max over the edges of y = s*act(z) + t picks the edge of largest act(z) when s > 0, of smallest when
+    s < 0, and the first edge when s == 0 (gamma = 0: every y equals t, an exact tie that torch.max and the
+    kernel both give to edge 0, so it is never masked).  The kernel ranks act(z) with the sign of s in every mode
+    (edge_bwd_kernel), and its fp32
     error lives in z, so the gap is measured there: on v = sign(s) * act(z), not on y, where a channel with
     gamma near 0 would tie everywhere although its edges are well apart.  An entry is masked when another
     edge's v is within TIE_REL * max(1, |v|) of the top - unless every edge that close sits robustly in ReLU's
@@ -63,12 +65,14 @@ def edge_tie_mask(x, edge_index, gconv_nn, act, norm, training):
     p = od.params_from_module(gconv_nn, dtype=torch.float64)
     z = _pre_activation(x, edge_index, p, "edge")
     v = od.activation(z, act, p.get("slope"))
+    sign = torch.ones_like(z[:, :, :1, :1])
     if norm is not None and str(norm).lower() == "batch":
-        v = v * torch.where(p["norm"]["weight"] >= 0, 1.0, -1.0).to(v.dtype).view(1, -1, 1, 1)
+        sign = torch.sign(p["norm"]["weight"]).to(v.dtype).view(1, -1, 1, 1)
+    v = v * sign
     top, arg = v.max(-1, keepdim=True)
     close = (top - v) < TIE_REL * top.abs().clamp_min(1.0)
     flat = (z < -TIE_REL * z.abs().clamp_min(1.0)) if str(act).lower() == "relu" else torch.zeros_like(close)
-    tie = (close.sum(-1, keepdim=True) > 1) & (close & ~flat).any(-1, keepdim=True)
+    tie = (close.sum(-1, keepdim=True) > 1) & (close & ~flat).any(-1, keepdim=True) & (sign != 0)
     mask = tie | _kink(z.gather(-1, arg), act)
     frac = mask.double().mean().item()
     assert frac <= MAX_MASKED, "near-tie mask covers %.2e of the entries" % frac

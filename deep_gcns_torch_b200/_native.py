@@ -133,9 +133,11 @@ _lock = threading.Lock()
 def _declare(lib):
     vp, sz = ctypes.c_void_p, ctypes.c_size_t
     lib.dgcn_version.restype = ctypes.c_int
+    lib.dgcn_version.argtypes = []
     lib.dgcn_status_string.restype = ctypes.c_char_p
     lib.dgcn_status_string.argtypes = [ctypes.c_int]
     lib.dgcn_last_cuda_error.restype = ctypes.c_char_p
+    lib.dgcn_last_cuda_error.argtypes = []
     lib.dgcn_knn_graph_workspace_bytes.restype = sz
     lib.dgcn_knn_graph_workspace_bytes.argtypes = [c_i64] * 4
     lib.dgcn_knn_graph.restype = ctypes.c_int
@@ -145,44 +147,27 @@ def _declare(lib):
     lib.dgcn_graph_conv_workspace_bytes.argtypes = [c_i32] + [c_i64] * 5
     lib.dgcn_graph_conv_forward.restype = ctypes.c_int
     lib.dgcn_graph_conv_forward.argtypes = [c_i32, vp, c_i64, c_i64, c_i64, c_i64, c_i64, vp, vp, c_i64,
-                                            ctypes.POINTER(BasicConvC), c_i64, vp, vp, sz, vp]
+                                            ctypes.POINTER(BasicConvC), c_i64, vp, ctypes.POINTER(BnSyncC), vp, sz, vp]
     lib.dgcn_dyn_conv_workspace_bytes.restype = sz
     lib.dgcn_dyn_conv_workspace_bytes.argtypes = [c_i32] + [c_i64] * 5
     lib.dgcn_dyn_conv_forward.restype = ctypes.c_int
     lib.dgcn_dyn_conv_forward.argtypes = [c_i32, vp, c_i64, c_i64, c_i64, c_i64, c_i64, ctypes.POINTER(DilationC),
-                                          ctypes.POINTER(BasicConvC), c_i64, vp, vp, vp, sz, vp]
-    lib.dgcn_dyn_conv_forward_fused.restype = ctypes.c_int
-    lib.dgcn_dyn_conv_forward_fused.argtypes = [c_i32, vp, c_i64, c_i64, c_i64, c_i64, c_i64, ctypes.POINTER(DilationC),
-                                                ctypes.POINTER(BasicConvC), c_i64, vp, vp, ctypes.POINTER(BlockFusionC),
-                                                vp, sz, vp]
-    lib.dgcn_graph_conv_forward_sync.restype = ctypes.c_int
-    lib.dgcn_graph_conv_forward_sync.argtypes = [c_i32, vp, c_i64, c_i64, c_i64, c_i64, c_i64, vp, vp, c_i64,
-                                                 ctypes.POINTER(BasicConvC), c_i64, vp, ctypes.POINTER(BnSyncC), vp, sz,
-                                                 vp]
-    lib.dgcn_dyn_conv_forward_sync.restype = ctypes.c_int
-    lib.dgcn_dyn_conv_forward_sync.argtypes = [c_i32, vp, c_i64, c_i64, c_i64, c_i64, c_i64, ctypes.POINTER(DilationC),
-                                               ctypes.POINTER(BasicConvC), c_i64, vp, vp, ctypes.POINTER(BnSyncC), vp,
-                                               sz, vp]
-    lib.dgcn_graph_conv_backward_sync.restype = ctypes.c_int
-    lib.dgcn_graph_conv_backward_sync.argtypes = [c_i32, vp, c_i64, c_i64, c_i64, c_i64, c_i64, vp, vp, c_i64,
-                                                  ctypes.POINTER(BasicConvC), c_i64, vp, vp, vp, vp, vp, vp, vp,
-                                                  ctypes.POINTER(BnSyncC), vp, sz, vp]
+                                          ctypes.POINTER(BasicConvC), c_i64, vp, vp, ctypes.POINTER(BlockFusionC),
+                                          ctypes.POINTER(BnSyncC), vp, sz, vp]
     lib.dgcn_graph_conv_backward_workspace_bytes.restype = sz
     lib.dgcn_graph_conv_backward_workspace_bytes.argtypes = [c_i32] + [c_i64] * 5
     lib.dgcn_graph_conv_backward.restype = ctypes.c_int
     lib.dgcn_graph_conv_backward.argtypes = [c_i32, vp, c_i64, c_i64, c_i64, c_i64, c_i64, vp, vp, c_i64,
                                              ctypes.POINTER(BasicConvC), c_i64, vp, vp, vp, vp, vp, vp, vp,
-                                             vp, sz, vp]
+                                             ctypes.POINTER(BnSyncC), vp, sz, vp]
     lib.dgcn_csr_build_workspace_bytes.restype = sz
     lib.dgcn_csr_build_workspace_bytes.argtypes = [c_i64, c_i64]
     lib.dgcn_csr_build.restype = ctypes.c_int
     lib.dgcn_csr_build.argtypes = [vp, c_i64, c_i64, vp, vp, vp, vp, sz, vp]
     lib.dgcn_genconv_aggregate.restype = ctypes.c_int
-    lib.dgcn_genconv_aggregate.argtypes = [vp, vp, c_i64, c_i64, vp, vp, vp, vp, ctypes.POINTER(GenconvParamsC),
-                                           ctypes.POINTER(CsrHubsC), vp, vp]
-    lib.dgcn_genconv_aggregate_fused.restype = ctypes.c_int
-    lib.dgcn_genconv_aggregate_fused.argtypes = [vp, vp, c_i64, c_i64, vp, vp, vp, vp, ctypes.POINTER(GenconvParamsC),
-                                                 ctypes.POINTER(CsrHubsC), ctypes.POINTER(GenconvFusionC), vp, vp]
+    lib.dgcn_genconv_aggregate.argtypes = [c_i32, vp, vp, c_i64, c_i64, vp, vp, vp, vp, ctypes.POINTER(GenconvParamsC),
+                                           ctypes.POINTER(CsrHubsC), ctypes.POINTER(GenconvFusionC),
+                                           ctypes.POINTER(KeepMaskC), vp, vp]
     lib.dgcn_linear_residual_workspace_bytes.restype = sz
     lib.dgcn_linear_residual_workspace_bytes.argtypes = [c_i64, c_i64]
     lib.dgcn_linear_residual.restype = ctypes.c_int
@@ -190,8 +175,9 @@ def _declare(lib):
     lib.dgcn_csr_hub_rows.restype = ctypes.c_int
     lib.dgcn_csr_hub_rows.argtypes = [vp, c_i64, c_i64, c_i32, c_i32, vp, vp, vp, vp]
     lib.dgcn_genconv_aggregate_backward.restype = ctypes.c_int
-    lib.dgcn_genconv_aggregate_backward.argtypes = [vp, vp, c_i64, c_i64, c_i64, vp, vp, vp, vp,
-                                                    ctypes.POINTER(GenconvParamsC), c_i32, vp, vp, vp, vp, vp, vp]
+    lib.dgcn_genconv_aggregate_backward.argtypes = [c_i32, vp, vp, c_i64, c_i64, c_i64, vp, vp, vp, vp,
+                                                    ctypes.POINTER(GenconvParamsC), c_i32, vp, vp, c_i32,
+                                                    ctypes.POINTER(KeepMaskC), vp, vp, vp, vp, vp, vp]
     lib.dgcn_debug_kernel_timing.restype = ctypes.c_int
     lib.dgcn_debug_kernel_timing.argtypes = [c_i32]
     lib.dgcn_debug_kernel_timing_read.restype = ctypes.c_int
@@ -202,24 +188,7 @@ def _declare(lib):
     lib.dgcn_debug_tc_certification_read.restype = ctypes.c_int
     lib.dgcn_debug_tc_certification_read.argtypes = [ctypes.POINTER(c_i64), ctypes.POINTER(c_i64)]
     lib.dgcn_gather_rows.restype = ctypes.c_int
-    lib.dgcn_gather_rows.argtypes = [vp, c_i64, vp, c_i64, vp, vp]
-    lib.dgcn_genconv_aggregate_fused_rows.restype = ctypes.c_int
-    lib.dgcn_genconv_aggregate_fused_rows.argtypes = [c_i32, vp, vp, c_i64, c_i64, vp, vp, vp, vp,
-                                                      ctypes.POINTER(GenconvParamsC), ctypes.POINTER(CsrHubsC),
-                                                      ctypes.POINTER(GenconvFusionC), vp, vp]
-    lib.dgcn_genconv_aggregate_backward_rows.restype = ctypes.c_int
-    lib.dgcn_genconv_aggregate_backward_rows.argtypes = [c_i32, vp, vp, c_i64, c_i64, c_i64, vp, vp, vp, vp,
-                                                         ctypes.POINTER(GenconvParamsC), c_i32, vp, vp, vp, vp, vp, vp]
-    lib.dgcn_gather_rows_typed.restype = ctypes.c_int
-    lib.dgcn_gather_rows_typed.argtypes = [c_i32, vp, c_i64, vp, c_i64, vp, vp]
-    lib.dgcn_genconv_aggregate_fused_keep.restype = ctypes.c_int
-    lib.dgcn_genconv_aggregate_fused_keep.argtypes = [c_i32, vp, vp, c_i64, c_i64, vp, vp, vp, vp,
-                                                      ctypes.POINTER(GenconvParamsC), ctypes.POINTER(CsrHubsC),
-                                                      ctypes.POINTER(GenconvFusionC), ctypes.POINTER(KeepMaskC), vp, vp]
-    lib.dgcn_genconv_aggregate_backward_keep.restype = ctypes.c_int
-    lib.dgcn_genconv_aggregate_backward_keep.argtypes = [c_i32, vp, vp, c_i64, c_i64, c_i64, vp, vp, vp, vp,
-                                                         ctypes.POINTER(GenconvParamsC), c_i32, vp, vp, c_i32,
-                                                         ctypes.POINTER(KeepMaskC), vp, vp, vp, vp, vp, vp]
+    lib.dgcn_gather_rows.argtypes = [c_i32, vp, c_i64, vp, c_i64, vp, vp]
     lib.dgcn_keep_bits_pack.restype = ctypes.c_int
     lib.dgcn_keep_bits_pack.argtypes = [vp, c_i64, c_i64, vp, vp]
     lib.dgcn_res_plus_backward_gy.restype = ctypes.c_int
@@ -357,15 +326,19 @@ class ConvParams:
     def tensors(self):
         return (self.weight, self.bias, self.prelu_weight, self.bn_weight, self.bn_bias, self.bn_mean, self.bn_var)
 
-    def c_struct(self, dev):
+    def c_struct(self, dev, stats=None):
+        """dgcn_basic_conv of these tensors.  stats None (forward): bn_mean / bn_var are the running statistics, and
+        in train mode new batch_mean / batch_var tensors receive the batch statistics.  stats = (mean, var)
+        (backward): the statistics the forward normalised with; nothing is allocated."""
         c_out = self.weight.shape[0]
         s = BasicConvC()
         s.weight, s.bias = _ptr(self.weight), _ptr(self.bias)
         s.act, s.slope, s.prelu_weight = self.act, 0.2, _ptr(self.prelu_weight)
         s.norm = self.norm
         s.bn_weight, s.bn_bias = _ptr(self.bn_weight), _ptr(self.bn_bias)
-        s.bn_mean, s.bn_var, s.bn_eps = _ptr(self.bn_mean), _ptr(self.bn_var), self.bn_eps
-        if self.norm == NORM_BATCH_TRAIN:
+        mean, var = (self.bn_mean, self.bn_var) if stats is None else stats
+        s.bn_mean, s.bn_var, s.bn_eps = _ptr(mean), _ptr(var), self.bn_eps
+        if stats is None and self.norm == NORM_BATCH_TRAIN:
             self.batch_mean = torch.empty(c_out, dtype=torch.float32, device=dev)
             self.batch_var = torch.empty(c_out, dtype=torch.float32, device=dev)
             s.batch_mean_out, s.batch_var_out = _ptr(self.batch_mean), _ptr(self.batch_var)
@@ -412,21 +385,17 @@ def graph_conv_forward(conv, x, prm, edge_index=None, nbr=None):
         out = torch.empty((B, c_out, N, 1), dtype=torch.float32, device=dev)
         ws = _workspace(l.dgcn_graph_conv_workspace_bytes(CONV[conv], B, C, c_out, N, k), dev)
         bs = prm.bn_sync(dev)
-        if bs is None:
-            rc = l.dgcn_graph_conv_forward(CONV[conv], _ptr(x3), B, C, N, sb, sc, _ptr(edge_index), _ptr(nbr), k,
-                                           ctypes.byref(cs), c_out, _ptr(out), _ptr(ws), ws.numel(), _stream(dev))
-            _check(rc, "dgcn_graph_conv_forward")
-        else:
-            rc = l.dgcn_graph_conv_forward_sync(CONV[conv], _ptr(x3), B, C, N, sb, sc, _ptr(edge_index), _ptr(nbr), k,
-                                                ctypes.byref(cs), c_out, _ptr(out), ctypes.byref(bs.c), _ptr(ws),
-                                                ws.numel(), _stream(dev))
-            bs.check(rc, "dgcn_graph_conv_forward_sync")
+        rc = l.dgcn_graph_conv_forward(CONV[conv], _ptr(x3), B, C, N, sb, sc, _ptr(edge_index), _ptr(nbr), k,
+                                       ctypes.byref(cs), c_out, _ptr(out), None if bs is None else ctypes.byref(bs.c),
+                                       _ptr(ws), ws.numel(), _stream(dev))
+        (_check if bs is None else bs.check)(rc, "dgcn_graph_conv_forward")
+        if bs is not None:
             prm.moments = bs.moments
     return out
 
 
 def dyn_conv_forward(conv, x, prm, k, dilation=1, cols=None, want_nbr=False, residual=None, res_scale=1.0, out=None):
-    """dgcn_dyn_conv_forward(_fused): (out (B, C_out, N, 1), nbr (B,N,k) int32 | None).
+    """dgcn_dyn_conv_forward: (out (B, C_out, N, 1), nbr (B,N,k) int32 | None).
 
     residual (B, C_out, N[, 1]): out = conv + residual * res_scale (ResDynBlock2d); out: write into this tensor, which
     may be a channel slice of a wider (B, C_total, N, 1) buffer (inference only, no train-mode BatchNorm)."""
@@ -459,19 +428,13 @@ def dyn_conv_forward(conv, x, prm, k, dilation=1, cols=None, want_nbr=False, res
         nbr = torch.empty((B, N, k), dtype=torch.int32, device=dev) if want_nbr else None
         ws = _workspace(l.dgcn_dyn_conv_workspace_bytes(CONV[conv], B, C, c_out, N, K), dev)
         bs = prm.bn_sync(dev)
-        if bs is None:
-            rc = l.dgcn_dyn_conv_forward_fused(CONV[conv], _ptr(x3), B, C, N, sb, sc, ctypes.byref(dil),
-                                               ctypes.byref(cs), c_out, _ptr(out), _ptr(nbr),
-                                               ctypes.byref(fus) if fus is not None else None, _ptr(ws), ws.numel(),
-                                               _stream(dev))
-            _check(rc, "dgcn_dyn_conv_forward")
-        else:
-            if fus is not None:
-                raise RuntimeError("dyn_conv_forward: the block epilogue does not run with train-mode BatchNorm")
-            rc = l.dgcn_dyn_conv_forward_sync(CONV[conv], _ptr(x3), B, C, N, sb, sc, ctypes.byref(dil),
-                                              ctypes.byref(cs), c_out, _ptr(out), _ptr(nbr), ctypes.byref(bs.c),
-                                              _ptr(ws), ws.numel(), _stream(dev))
-            bs.check(rc, "dgcn_dyn_conv_forward_sync")
+        if bs is not None and fus is not None:
+            raise RuntimeError("dyn_conv_forward: the block epilogue does not run with train-mode BatchNorm")
+        rc = l.dgcn_dyn_conv_forward(CONV[conv], _ptr(x3), B, C, N, sb, sc, ctypes.byref(dil), ctypes.byref(cs), c_out,
+                                     _ptr(out), _ptr(nbr), None if fus is None else ctypes.byref(fus),
+                                     None if bs is None else ctypes.byref(bs.c), _ptr(ws), ws.numel(), _stream(dev))
+        (_check if bs is None else bs.check)(rc, "dgcn_dyn_conv_forward")
+        if bs is not None:
             prm.moments = bs.moments
     return out, nbr
 
@@ -491,15 +454,9 @@ def graph_conv_backward(conv, x, prm, grad_out, edge_index=None, nbr=None, need_
         k = nbr.shape[-1]
     with torch.cuda.device(dev):
         l = lib()
-        cs = BasicConvC()
-        cs.weight, cs.bias = _ptr(prm.weight), _ptr(prm.bias)
-        cs.act, cs.slope, cs.prelu_weight = prm.act, 0.2, _ptr(prm.prelu_weight)
-        cs.norm = prm.norm
-        cs.bn_weight, cs.bn_bias, cs.bn_eps = _ptr(prm.bn_weight), _ptr(prm.bn_bias), prm.bn_eps
-        if prm.norm == NORM_BATCH_TRAIN:      # statistics of the batch the forward normalised with
-            cs.bn_mean, cs.bn_var = _ptr(prm.batch_mean), _ptr(prm.batch_var)
-        else:
-            cs.bn_mean, cs.bn_var = _ptr(prm.bn_mean), _ptr(prm.bn_var)
+        # train mode: the statistics of the batch the forward normalised with
+        stats = (prm.batch_mean, prm.batch_var) if prm.norm == NORM_BATCH_TRAIN else (prm.bn_mean, prm.bn_var)
+        cs = prm.c_struct(dev, stats)
         f = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)
         g = {"x": f(B, C, N) if need_x else None, "weight": f(c_out, 2 * C),
              "bias": f(c_out) if prm.bias is not None else None,
@@ -510,16 +467,11 @@ def graph_conv_backward(conv, x, prm, grad_out, edge_index=None, nbr=None, need_
         bs = prm.bn_sync(dev)
         grads = (_ptr(g["x"]), _ptr(g["weight"]), _ptr(g["bias"]), _ptr(g["bn_weight"]), _ptr(g["bn_bias"]),
                  _ptr(g["prelu"]))
-        if bs is None:
-            rc = l.dgcn_graph_conv_backward(CONV[conv], _ptr(x3), B, C, N, sb, sc, _ptr(edge_index), _ptr(nbr), k,
-                                            ctypes.byref(cs), c_out, _ptr(go), *grads, _ptr(ws), ws.numel(),
-                                            _stream(dev))
-            _check(rc, "dgcn_graph_conv_backward")
-        else:       # dx from the cross-rank sums; the parameter gradients stay local (SyncBatchNorm)
-            rc = l.dgcn_graph_conv_backward_sync(CONV[conv], _ptr(x3), B, C, N, sb, sc, _ptr(edge_index), _ptr(nbr), k,
-                                                 ctypes.byref(cs), c_out, _ptr(go), *grads, ctypes.byref(bs.c),
-                                                 _ptr(ws), ws.numel(), _stream(dev))
-            bs.check(rc, "dgcn_graph_conv_backward_sync")
+        # synced: dx from the cross-rank sums; the parameter gradients stay local (SyncBatchNorm)
+        rc = l.dgcn_graph_conv_backward(CONV[conv], _ptr(x3), B, C, N, sb, sc, _ptr(edge_index), _ptr(nbr), k,
+                                        ctypes.byref(cs), c_out, _ptr(go), *grads,
+                                        None if bs is None else ctypes.byref(bs.c), _ptr(ws), ws.numel(), _stream(dev))
+        (_check if bs is None else bs.check)(rc, "dgcn_graph_conv_backward")
     return g
 
 
@@ -595,7 +547,7 @@ def _keep_mask(keep):
 
 def genconv_aggregate(x_src, x_dst, csr, prm, edge_attr=None, out=None, pre=None, rows=None, skip_hubs=False,
                       keep=None):
-    """dgcn_genconv_aggregate(_fused / _fused_keep): out (N, C) = x_dst + MsgNorm(aggregate(message)).
+    """dgcn_genconv_aggregate: out (N, C) = x_dst + MsgNorm(aggregate(message)).
 
     out: write into this (N, C) tensor (e.g. a view of a persistent buffer) instead of a new one.
     pre = (scale (C), shift (C), relu): rows of x_src / x_dst are read as act(scale * x + shift).
@@ -633,19 +585,18 @@ def genconv_aggregate(x_src, x_dst, csr, prm, edge_attr=None, out=None, pre=None
                 fus.row_list, fus.n_rows = (rows.data_ptr() or None), rows.numel()
                 if rows.numel() == 0 and skip_hubs:
                     return out
-        rc = lib().dgcn_genconv_aggregate_fused_keep(dtype, _ptr(x_src), _ptr(x_dst), N, C, _ptr(rowptr), _ptr(src),
-                                                     _ptr(eid), _ptr(edge_attr), ctypes.byref(prm),
-                                                     ctypes.byref(hubs) if hubs is not None else None,
-                                                     ctypes.byref(fus) if fus is not None else None,
-                                                     ctypes.byref(km) if km is not None else None, _ptr(out),
-                                                     _stream(dev))
+        rc = lib().dgcn_genconv_aggregate(dtype, _ptr(x_src), _ptr(x_dst), N, C, _ptr(rowptr), _ptr(src), _ptr(eid),
+                                          _ptr(edge_attr), ctypes.byref(prm),
+                                          ctypes.byref(hubs) if hubs is not None else None,
+                                          ctypes.byref(fus) if fus is not None else None,
+                                          ctypes.byref(km) if km is not None else None, _ptr(out), _stream(dev))
         _check(rc, "dgcn_genconv_aggregate")
     return out
 
 
 def genconv_aggregate_backward(x_src, x_dst, csr, prm, grad_out, edge_attr=None, softmax_grad=False,
                                need_edge_attr=False, pre=None, keep=None):
-    """dgcn_genconv_aggregate_backward(_rows / _keep): (grad_x_src (N_src,C) fp32, grad_x_dst (N,C) fp32 | None,
+    """dgcn_genconv_aggregate_backward: (grad_x_src (N_src,C) fp32, grad_x_dst (N,C) fp32 | None,
     grad_edge_attr in edge_attr's row dtype | None, grad_scalars (4) = d/dt, d/dp, d/dy, d/dmsg_scale).
     pre / keep: the forward's (genconv_aggregate); the row gradients are then w.r.t. the activated rows."""
     rowptr, src, eid = csr[:3]
@@ -668,12 +619,12 @@ def genconv_aggregate_backward(x_src, x_dst, csr, prm, grad_out, edge_attr=None,
             full = dtype != DTYPE_F32 and edge_attr.shape[0] == src.numel() and edge_attr.shape[0] > 1
             gea = torch.empty_like(edge_attr) if full else torch.zeros_like(edge_attr)
         gsc = torch.zeros(4, dtype=torch.float32, device=dev)
-        rc = lib().dgcn_genconv_aggregate_backward_keep(dtype, _ptr(x_src), _ptr(x_dst), N, x_src.shape[0], C,
-                                                        _ptr(rowptr), _ptr(src), _ptr(eid), _ptr(edge_attr),
-                                                        ctypes.byref(prm), int(bool(softmax_grad)), _ptr(ps), _ptr(ph),
-                                                        int(bool(pre[2])) if pre is not None else 0,
-                                                        ctypes.byref(km) if km is not None else None, _ptr(grad_out),
-                                                        _ptr(gsrc), _ptr(gdst), _ptr(gea), _ptr(gsc), _stream(dev))
+        rc = lib().dgcn_genconv_aggregate_backward(dtype, _ptr(x_src), _ptr(x_dst), N, x_src.shape[0], C,
+                                                   _ptr(rowptr), _ptr(src), _ptr(eid), _ptr(edge_attr),
+                                                   ctypes.byref(prm), int(bool(softmax_grad)), _ptr(ps), _ptr(ph),
+                                                   int(bool(pre[2])) if pre is not None else 0,
+                                                   ctypes.byref(km) if km is not None else None, _ptr(grad_out),
+                                                   _ptr(gsrc), _ptr(gdst), _ptr(gea), _ptr(gsc), _stream(dev))
         _check(rc, "dgcn_genconv_aggregate_backward")
     return gsrc, gdst, gea, gsc
 
@@ -754,8 +705,8 @@ def gather_rows(x, rows, out=None):
             out = torch.empty((R, C), dtype=x.dtype, device=x.device)
         elif out.dtype != x.dtype or out.shape != (R, C) or not out.is_contiguous():
             raise RuntimeError("gather_rows: out must be a contiguous (R, C) tensor of x's dtype")
-        _check(lib().dgcn_gather_rows_typed(dtype, _ptr(x), C, _ptr(rows), R, _ptr(out), _stream(x.device)),
-               "dgcn_gather_rows_typed")
+        _check(lib().dgcn_gather_rows(dtype, _ptr(x), C, _ptr(rows), R, _ptr(out), _stream(x.device)),
+               "dgcn_gather_rows")
     return out
 
 

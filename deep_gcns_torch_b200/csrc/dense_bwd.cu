@@ -402,7 +402,7 @@ __global__ void mr_scatter_kernel(const float* __restrict__ dxcat, const int32_t
   atomicAdd(row + arg_i[t], -dr);
 }
 
-// The regions of dgcn_graph_conv_backward_sync, in the order it uses them.
+// The regions of dgcn_graph_conv_backward, in the order it uses them.
 struct BwdRegions {
   int64_t n_partial;         // statistic rows: one per CTA of edge_bwd_kernel / mr_bn_bwd_kernel
   float* wk;                 // packed weights
@@ -455,19 +455,8 @@ size_t dgcn_graph_conv_backward_workspace_bytes(int32_t conv, int64_t B, int64_t
 int dgcn_graph_conv_backward(int32_t conv, const float* x, int64_t B, int64_t ci, int64_t N, int64_t sb, int64_t sc,
                              const int64_t* edge_index, const int32_t* nbr, int64_t k, const dgcn_basic_conv* p,
                              int64_t co, const float* grad_out, float* grad_x, float* grad_weight, float* grad_bias,
-                             float* grad_bn_weight, float* grad_bn_bias, float* grad_prelu, void* wsp, size_t ws_bytes,
-                             dgcn_stream_t stream_) {
-  return dgcn_graph_conv_backward_sync(conv, x, B, ci, N, sb, sc, edge_index, nbr, k, p, co, grad_out, grad_x,
-                                       grad_weight, grad_bias, grad_bn_weight, grad_bn_bias, grad_prelu, nullptr, wsp,
-                                       ws_bytes, stream_);
-}
-
-int dgcn_graph_conv_backward_sync(int32_t conv, const float* x, int64_t B, int64_t ci, int64_t N, int64_t sb,
-                                  int64_t sc, const int64_t* edge_index, const int32_t* nbr, int64_t k,
-                                  const dgcn_basic_conv* p, int64_t co, const float* grad_out, float* grad_x,
-                                  float* grad_weight, float* grad_bias, float* grad_bn_weight, float* grad_bn_bias,
-                                  float* grad_prelu, const dgcn_bn_sync* sync, void* wsp, size_t ws_bytes,
-                                  dgcn_stream_t stream_) {
+                             float* grad_bn_weight, float* grad_bn_bias, float* grad_prelu, const dgcn_bn_sync* sync,
+                             void* wsp, size_t ws_bytes, dgcn_stream_t stream_) {
   if (conv != DGCN_CONV_EDGE && conv != DGCN_CONV_MR) return DGCN_ERR_UNSUPPORTED;
   if (!x || !p || !p->weight || !grad_out || (!edge_index && !nbr) || B <= 0 || ci <= 0 || co <= 0 || N <= 0 || k <= 0)
     return DGCN_ERR_BAD_ARG;

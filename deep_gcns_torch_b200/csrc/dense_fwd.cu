@@ -949,16 +949,8 @@ size_t dgcn_graph_conv_workspace_bytes(int32_t conv, int64_t B, int64_t C_in, in
 
 int dgcn_graph_conv_forward(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N, int64_t stride_b,
                             int64_t stride_c, const int64_t* edge_index, const int32_t* nbr, int64_t k,
-                            const dgcn_basic_conv* p, int64_t C_out, float* out, void* wsp, size_t ws_bytes,
-                            dgcn_stream_t stream) {
-  return dgcn_graph_conv_forward_sync(conv, x, B, C_in, N, stride_b, stride_c, edge_index, nbr, k, p, C_out, out,
-                                      nullptr, wsp, ws_bytes, stream);
-}
-
-int dgcn_graph_conv_forward_sync(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N, int64_t stride_b,
-                                 int64_t stride_c, const int64_t* edge_index, const int32_t* nbr, int64_t k,
-                                 const dgcn_basic_conv* p, int64_t C_out, float* out, const dgcn_bn_sync* sync,
-                                 void* wsp, size_t ws_bytes, dgcn_stream_t stream) {
+                            const dgcn_basic_conv* p, int64_t C_out, float* out, const dgcn_bn_sync* sync, void* wsp,
+                            size_t ws_bytes, dgcn_stream_t stream) {
   int rc = check_conv_args(conv, x, B, C_in, N, p, C_out, out);
   if (rc != DGCN_OK) return rc;
   if ((!edge_index && !nbr) || k <= 0) return DGCN_ERR_BAD_ARG;
@@ -977,34 +969,15 @@ size_t dgcn_dyn_conv_workspace_bytes(int32_t conv, int64_t B, int64_t C_in, int6
 
 int dgcn_dyn_conv_forward(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N, int64_t stride_b,
                           int64_t stride_c, const dgcn_dilation* dil, const dgcn_basic_conv* p, int64_t C_out,
-                          float* out, int32_t* nbr_out, void* wsp, size_t ws_bytes, dgcn_stream_t stream) {
-  return dgcn_dyn_conv_forward_sync(conv, x, B, C_in, N, stride_b, stride_c, dil, p, C_out, out, nbr_out, nullptr, wsp,
-                                    ws_bytes, stream);
-}
-
-int dgcn_dyn_conv_forward_fused(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N, int64_t stride_b,
-                                int64_t stride_c, const dgcn_dilation* dil, const dgcn_basic_conv* p, int64_t C_out,
-                                float* out, int32_t* nbr_out, const dgcn_block_fusion* fus, void* wsp, size_t ws_bytes,
-                                dgcn_stream_t stream) {
-  int rc = check_conv_args(conv, x, B, C_in, N, p, C_out, out);
-  if (rc != DGCN_OK) return rc;
-  if (!dil) return DGCN_ERR_BAD_ARG;
-  Workspace ws(wsp, ws_bytes);
-  return conv_forward(conv, x, B, C_in, N, stride_b, stride_c, nullptr, nullptr, 0, dil, p, C_out, out, nbr_out, ws,
-                      static_cast<cudaStream_t>(stream), fus, nullptr);
-}
-
-int dgcn_dyn_conv_forward_sync(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N, int64_t stride_b,
-                               int64_t stride_c, const dgcn_dilation* dil, const dgcn_basic_conv* p, int64_t C_out,
-                               float* out, int32_t* nbr_out, const dgcn_bn_sync* sync, void* wsp, size_t ws_bytes,
-                               dgcn_stream_t stream) {
+                          float* out, int32_t* nbr_out, const dgcn_block_fusion* fus, const dgcn_bn_sync* sync,
+                          void* wsp, size_t ws_bytes, dgcn_stream_t stream) {
   int rc = check_conv_args(conv, x, B, C_in, N, p, C_out, out);
   if (rc != DGCN_OK) return rc;
   if (!dil) return DGCN_ERR_BAD_ARG;
   if (sync && (!sync->moments || !sync->reduce)) return DGCN_ERR_BAD_ARG;
   Workspace ws(wsp, ws_bytes);
   return conv_forward(conv, x, B, C_in, N, stride_b, stride_c, nullptr, nullptr, 0, dil, p, C_out, out, nbr_out, ws,
-                      static_cast<cudaStream_t>(stream), nullptr, sync);
+                      static_cast<cudaStream_t>(stream), fus, sync);
 }
 
 }  // extern "C"

@@ -254,36 +254,14 @@ static void launch_bwd(const AggrBwdArgs& g, cudaStream_t s) {
 
 using namespace dgcn;
 
-extern "C" int dgcn_genconv_aggregate_backward(const float* x_src, const float* x_dst, int64_t N, int64_t N_src,
-                                               int64_t C, const int32_t* rowptr, const int32_t* src,
-                                               const int32_t* eid, const float* edge_attr,
+extern "C" int dgcn_genconv_aggregate_backward(int32_t dtype, const void* x_src, const void* x_dst, int64_t N,
+                                               int64_t N_src, int64_t C, const int32_t* rowptr, const int32_t* src,
+                                               const int32_t* eid, const void* edge_attr,
                                                const dgcn_genconv_params* prm, int32_t softmax_grad,
-                                               const float* grad_out, float* grad_x_src, float* grad_x_dst,
-                                               float* grad_edge_attr, float* grad_scalars, dgcn_stream_t stream) {
-  return dgcn_genconv_aggregate_backward_rows(DGCN_F32, x_src, x_dst, N, N_src, C, rowptr, src, eid, edge_attr, prm,
-                                              softmax_grad, grad_out, grad_x_src, grad_x_dst, grad_edge_attr,
-                                              grad_scalars, stream);
-}
-
-extern "C" int dgcn_genconv_aggregate_backward_rows(int32_t dtype, const void* x_src, const void* x_dst, int64_t N,
-                                                    int64_t N_src, int64_t C, const int32_t* rowptr,
-                                                    const int32_t* src, const int32_t* eid, const void* edge_attr,
-                                                    const dgcn_genconv_params* prm, int32_t softmax_grad,
-                                                    const float* grad_out, float* grad_x_src, float* grad_x_dst,
-                                                    void* grad_edge_attr, float* grad_scalars, dgcn_stream_t stream) {
-  return dgcn_genconv_aggregate_backward_keep(dtype, x_src, x_dst, N, N_src, C, rowptr, src, eid, edge_attr, prm,
-                                              softmax_grad, nullptr, nullptr, 0, nullptr, grad_out, grad_x_src,
-                                              grad_x_dst, grad_edge_attr, grad_scalars, stream);
-}
-
-extern "C" int dgcn_genconv_aggregate_backward_keep(int32_t dtype, const void* x_src, const void* x_dst, int64_t N,
-                                                    int64_t N_src, int64_t C, const int32_t* rowptr,
-                                                    const int32_t* src, const int32_t* eid, const void* edge_attr,
-                                                    const dgcn_genconv_params* prm, int32_t softmax_grad,
-                                                    const float* pre_scale, const float* pre_shift, int32_t pre_relu,
-                                                    const dgcn_keep_mask* keep, const float* grad_out,
-                                                    float* grad_x_src, float* grad_x_dst, void* grad_edge_attr,
-                                                    float* grad_scalars, dgcn_stream_t stream) {
+                                               const float* pre_scale, const float* pre_shift, int32_t pre_relu,
+                                               const dgcn_keep_mask* keep, const float* grad_out, float* grad_x_src,
+                                               float* grad_x_dst, void* grad_edge_attr, float* grad_scalars,
+                                               dgcn_stream_t stream) {
   (void)N_src;
   if (!x_src || !rowptr || !src || !prm || !grad_out || N < 0 || C <= 0) return DGCN_ERR_BAD_ARG;
   if (dtype != DGCN_F32 && dtype != DGCN_BF16 && dtype != DGCN_F16) return DGCN_ERR_BAD_ARG;

@@ -61,35 +61,10 @@ int dgcn_csr_hub_rows(const int32_t* rowptr, int64_t N, int64_t E, int32_t min_d
   return DGCN_OK;
 }
 
-int dgcn_genconv_aggregate(const float* x_src, const float* x_dst, int64_t N, int64_t C, const int32_t* rowptr,
-                           const int32_t* src, const int32_t* eid, const float* edge_attr,
-                           const dgcn_genconv_params* prm, const dgcn_csr_hubs* hubs, float* out,
-                           dgcn_stream_t stream) {
-  return dgcn_genconv_aggregate_fused(x_src, x_dst, N, C, rowptr, src, eid, edge_attr, prm, hubs, nullptr, out, stream);
-}
-
-int dgcn_genconv_aggregate_fused(const float* x_src, const float* x_dst, int64_t N, int64_t C, const int32_t* rowptr,
-                                 const int32_t* src, const int32_t* eid, const float* edge_attr,
-                                 const dgcn_genconv_params* prm, const dgcn_csr_hubs* hubs,
-                                 const dgcn_genconv_fusion* fus, float* out, dgcn_stream_t stream) {
-  return dgcn_genconv_aggregate_fused_rows(DGCN_F32, x_src, x_dst, N, C, rowptr, src, eid, edge_attr, prm, hubs, fus,
-                                           out, stream);
-}
-
-int dgcn_genconv_aggregate_fused_rows(int32_t dtype, const void* x_src, const void* x_dst, int64_t N, int64_t C,
-                                      const int32_t* rowptr, const int32_t* src, const int32_t* eid,
-                                      const void* edge_attr, const dgcn_genconv_params* prm,
-                                      const dgcn_csr_hubs* hubs, const dgcn_genconv_fusion* fus, float* out,
-                                      dgcn_stream_t stream) {
-  return dgcn_genconv_aggregate_fused_keep(dtype, x_src, x_dst, N, C, rowptr, src, eid, edge_attr, prm, hubs, fus,
-                                           nullptr, out, stream);
-}
-
-int dgcn_genconv_aggregate_fused_keep(int32_t dtype, const void* x_src, const void* x_dst, int64_t N, int64_t C,
-                                      const int32_t* rowptr, const int32_t* src, const int32_t* eid,
-                                      const void* edge_attr, const dgcn_genconv_params* prm,
-                                      const dgcn_csr_hubs* hubs, const dgcn_genconv_fusion* fus,
-                                      const dgcn_keep_mask* keep, float* out, dgcn_stream_t stream) {
+int dgcn_genconv_aggregate(int32_t dtype, const void* x_src, const void* x_dst, int64_t N, int64_t C,
+                           const int32_t* rowptr, const int32_t* src, const int32_t* eid, const void* edge_attr,
+                           const dgcn_genconv_params* prm, const dgcn_csr_hubs* hubs, const dgcn_genconv_fusion* fus,
+                           const dgcn_keep_mask* keep, float* out, dgcn_stream_t stream) {
   if (!x_src || !rowptr || !src || !prm || !out || N < 0 || C <= 0) return DGCN_ERR_BAD_ARG;
   if (dtype != DGCN_F32 && dtype != DGCN_BF16 && dtype != DGCN_F16) return DGCN_ERR_BAD_ARG;
   if (fus && ((fus->pre_scale == nullptr) != (fus->pre_shift == nullptr))) return DGCN_ERR_BAD_ARG;
@@ -165,12 +140,8 @@ int dgcn_genconv_aggregate_fused_keep(int32_t dtype, const void* x_src, const vo
   return DGCN_ERR_UNSUPPORTED;
 }
 
-int dgcn_gather_rows(const float* x, int64_t C, const int32_t* rows, int64_t R, float* out, dgcn_stream_t stream) {
-  return dgcn_gather_rows_typed(DGCN_F32, x, C, rows, R, out, stream);
-}
-
-int dgcn_gather_rows_typed(int32_t dtype, const void* x, int64_t C, const int32_t* rows, int64_t R, void* out,
-                           dgcn_stream_t stream) {
+int dgcn_gather_rows(int32_t dtype, const void* x, int64_t C, const int32_t* rows, int64_t R, void* out,
+                     dgcn_stream_t stream) {
   if (C <= 0 || R < 0) return DGCN_ERR_BAD_ARG;
   if (dtype != DGCN_F32 && dtype != DGCN_BF16 && dtype != DGCN_F16) return DGCN_ERR_BAD_ARG;
   if (R == 0) return DGCN_OK;   // an empty halo list is legal (its tensors have null data pointers)

@@ -1,4 +1,4 @@
-// Sparse path, forward on bf16 / fp16 rows (dgcn_genconv_aggregate_fused_rows): the aggregate kernel of
+// Sparse path, forward on bf16 / fp16 rows (dgcn_genconv_aggregate, DGCN_BF16 / DGCN_F16): the aggregate kernel of
 // sparse_aggr.cuh instantiated for half-precision x_src / x_dst / edge_attr.  A launch uses the (VEC, NBLK) the
 // fp32 dispatch picks for the same C, so the lane <-> channel mapping, and with it every fp32 sum (MsgNorm's
 // warp-reduced norms included), is the same as on the upcast rows: the output is bit-identical.  Only the loads

@@ -106,7 +106,7 @@ int dgcn_debug_tc_certification_read(int64_t* uncertified, int64_t* queries) {
   *queries = dgcn::g_cert_queries.exchange(0);
   return DGCN_OK;
 }
-int dgcn_version(void) { return 100; }
+int dgcn_version(void) { return 200; }
 const char* dgcn_status_string(int status) {
   switch (status) {
     case DGCN_OK: return "ok";

@@ -7,7 +7,7 @@ The reference writes the block as separate modules (examples/ogb/ogbn_arxiv/mode
 In eval mode the BatchNorm1d is a per-channel affine, dropout is the identity and GENConv with
 mlp_layers=1 ends in one Linear.  `res_plus_block` runs the same arithmetic in two launches:
 
-    dgcn_genconv_aggregate_fused   reads h rows as relu(s*h + t) (gathered rows and the residual row),
+    dgcn_genconv_aggregate         reads h rows as relu(s*h + t) (gathered rows and the residual row),
                                    message + aggregate + MsgNorm + (z_i + m_i)     -> a
     dgcn_linear_residual           h_out = h + a W^T + b on the tensor cores (wgmma; two-plane bf16 split of both
                                    operands, fp32 accumulation; bias and skip connection in the epilogue)

@@ -13,9 +13,9 @@ concatenated in steady state:
     xbuf = [ local rows (n_local, C) | halo rows (n_halo, C) ]     one buffer, written in place
     comm stream : dgcn_gather_rows(local rows peers asked for) -> send buffer
                   all_to_all_single(send -> xbuf[n_local:])        NCCL over NVLink, async
-    main stream : dgcn_genconv_aggregate_fused(rows = interior)    rows whose sources are all local
+    main stream : dgcn_genconv_aggregate(rows = interior)          rows whose sources are all local
                   wait(all_to_all)
-                  dgcn_genconv_aggregate_fused(rows = boundary)    rows that read halo rows (+ hub rows)
+                  dgcn_genconv_aggregate(rows = boundary)          rows that read halo rows (+ hub rows)
 
 The exchange is the only collective of the forward; BatchNorm1d (eval) / MLP are row-local.
 Training: `HaloExchange` / `PartitionedAggregate` are autograd nodes, the backward of the

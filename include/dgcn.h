@@ -8,7 +8,7 @@
  *
  * Conventions
  *   - all pointers are DEVICE pointers unless the name ends in _host;
- *   - tensors are fp32 (the sparse *_rows / *_typed entry points also take bf16 / fp16
+ *   - tensors are fp32 (the sparse entry points with a `dtype` argument also take bf16 / fp16
  *     rows, dgcn_dtype), dense, in the reference's own layouts:
  *       dense path   x (B, C, N, 1)  -> element (b,c,n) at x[b*stride_b + c*stride_c + n]
  *                    edge_index (2, B, N, k) int64, plane 0 = neighbour j, plane 1 = centre i
@@ -49,7 +49,7 @@ enum dgcn_act { DGCN_ACT_NONE = 0, DGCN_ACT_RELU = 1, DGCN_ACT_LEAKYRELU = 2, DG
 enum dgcn_norm { DGCN_NORM_NONE = 0, DGCN_NORM_BATCH_EVAL = 1, DGCN_NORM_BATCH_TRAIN = 2 };
 /* gcn_lib/dense/torch_vertex.py:44-49 (GraphConv2d dispatch) */
 enum dgcn_conv { DGCN_CONV_EDGE = 0, DGCN_CONV_MR = 1 };
-/* Element type of the node / edge rows the sparse entry points read (the *_rows / *_typed variants).  bf16 and
+/* Element type of the node / edge rows the sparse entry points read (their `dtype` argument).  bf16 and
  * fp16 rows are widened to fp32 in registers (exact) and everything is computed in fp32 as for fp32 rows. */
 enum dgcn_dtype { DGCN_F32 = 0, DGCN_BF16 = 1, DGCN_F16 = 2 };
 /* gcn_lib/sparse/torch_message.py:44-85 (GenMessagePassing.aggregate) */
@@ -130,71 +130,10 @@ int dgcn_knn_graph(const float* x, int64_t B, int64_t C, int64_t N, int64_t stri
                    int64_t* edge_index, int32_t* nbr, void* ws, size_t ws_bytes,
                    dgcn_stream_t stream);
 
-/* Static graph convolution on a given graph.
- * Replaces gcn_lib/dense/torch_vertex.py:38-52 (GraphConv2d.forward) =
- * EdgeConv2d.forward :31-35 / MRConv2d.forward :16-20, including
- * batched_index_select (gcn_lib/dense/torch_nn.py:75-96) and BasicConv
- * (torch_nn.py:48-58: conv1x1 -> act -> norm) and the max over neighbours.
- * The graph comes either as the reference's int64 edge_index (2,B,N,k) with
- * arbitrary centres, or as nbr (B,N,k) int32 with centre = own index.
- * out: (B, C_out, N) contiguous. */
-size_t dgcn_graph_conv_workspace_bytes(int32_t conv, int64_t B, int64_t C_in, int64_t C_out,
-                                       int64_t N, int64_t k);
-int dgcn_graph_conv_forward(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N,
-                            int64_t stride_b, int64_t stride_c, const int64_t* edge_index,
-                            const int32_t* nbr, int64_t k, const dgcn_basic_conv* p,
-                            int64_t C_out, float* out, void* ws, size_t ws_bytes,
-                            dgcn_stream_t stream);
-
-/* Dynamic graph convolution: dilated kNN graph on x, then the convolution, in
- * one call; the neighbour list goes from the selection kernel's shared memory
- * straight into the gather/max and never reaches HBM unless nbr_out != NULL.
- * Replaces gcn_lib/dense/torch_vertex.py:55-72 (DynConv2d.forward with
- * knn='matrix'). */
-size_t dgcn_dyn_conv_workspace_bytes(int32_t conv, int64_t B, int64_t C_in, int64_t C_out,
-                                     int64_t N, int64_t K);
-int dgcn_dyn_conv_forward(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N,
-                          int64_t stride_b, int64_t stride_c, const dgcn_dilation* dil,
-                          const dgcn_basic_conv* p, int64_t C_out, float* out, int32_t* nbr_out,
-                          void* ws, size_t ws_bytes, dgcn_stream_t stream);
-
-/* Block epilogue around the dynamic convolution (SURVEY.md 8f rank 1), inference (no train-mode BatchNorm):
- *   residual != NULL: out = conv(x) + residual * res_scale   (ResDynBlock2d.forward, gcn_lib/dense/torch_vertex.py:101;
- *     residual (B, C_out, N) with strides res_stride_b / res_stride_c, unit stride along points)
- *   out_stride_b != 0: batch stride of `out` in floats - `out` is a channel slice of a wider (B, C_total, N) buffer
- *     (DenseDynBlock2d's torch.cat, :116, or a model's fusion buffer, examples/sem_seg_dense/architecture.py:52). */
-typedef struct dgcn_block_fusion {
-  const float* residual;
-  int64_t res_stride_b, res_stride_c;
-  float res_scale;
-  int64_t out_stride_b;
-} dgcn_block_fusion;
-int dgcn_dyn_conv_forward_fused(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N,
-                                int64_t stride_b, int64_t stride_c, const dgcn_dilation* dil,
-                                const dgcn_basic_conv* p, int64_t C_out, float* out, int32_t* nbr_out,
-                                const dgcn_block_fusion* fus /* may be NULL */, void* ws, size_t ws_bytes,
-                                dgcn_stream_t stream);
-
-/* Gradient of dgcn_graph_conv_forward w.r.t. x and the BasicConv parameters
- * (what torch autograd derives for torch_vertex.py:16-35 + torch_nn.py:48-58).
- * The graph is the one used in forward (edge_index (2,B,N,k) int64 or nbr
- * (B,N,k) int32 with centre = own index; the kNN graph itself is
- * non-differentiable, torch_edge.py:53-56).  With DGCN_NORM_BATCH_TRAIN,
- * p->bn_mean / p->bn_var must hold the BATCH statistics the forward returned.
- * grad_x is (B, C_in, N) contiguous.
- * grad_weight (C_out,2*C_in), grad_bias (C_out), grad_bn_weight/bias (C_out),
- * grad_prelu (1) are OVERWRITTEN; any of them may be NULL. */
-size_t dgcn_graph_conv_backward_workspace_bytes(int32_t conv, int64_t B, int64_t C_in,
-                                                int64_t C_out, int64_t N, int64_t k);
-int dgcn_graph_conv_backward(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N,
-                             int64_t stride_b, int64_t stride_c, const int64_t* edge_index,
-                             const int32_t* nbr, int64_t k,
-                             const dgcn_basic_conv* p, int64_t C_out, const float* grad_out,
-                             float* grad_x, float* grad_weight, float* grad_bias,
-                             float* grad_bn_weight, float* grad_bn_bias, float* grad_prelu,
-                             void* ws, size_t ws_bytes, dgcn_stream_t stream);
-
-/* Train-mode BatchNorm statistics shared across data-parallel ranks (torch.nn.SyncBatchNorm).
+/* Train-mode BatchNorm statistics shared across data-parallel ranks (torch.nn.SyncBatchNorm), the `sync`
+ * argument of dgcn_graph_conv_forward, dgcn_dyn_conv_forward and dgcn_graph_conv_backward.  sync == NULL, or a
+ * norm other than DGCN_NORM_BATCH_TRAIN: the statistics are the call's own (reduce is never called).  The
+ * workspace sizes do not depend on it.
  * moments: caller-owned DEVICE buffer of 2*C_out + 1 doubles.  Forward: [sum a | sum a^2 | count] over the
  *   positions this rank normalises (EdgeConv: the B*N*k edge activations, MRConv: the B*N node activations);
  *   backward: [sum g | sum g*ahat | count] over the same positions.
@@ -203,7 +142,7 @@ int dgcn_graph_conv_backward(int32_t conv, const float* x, int64_t B, int64_t C_
  *   element-wise sum of `moments` over all ranks (an all-reduce, in place) in the stream order of `stream` and
  *   return 0; it must not wait for the device.  Every rank has to make the same sequence of calls, so the
  *   all-reduces pair up.  A non-zero return abandons the call with DGCN_ERR_REDUCE (work already enqueued
- *   still runs; the outputs are undefined).
+ *   still runs; the outputs are undefined).  A sync with a NULL moments or reduce is DGCN_ERR_BAD_ARG.
  * After the reduce the library normalises with the GLOBAL mean and biased variance (forward) and forms grad_x
  * from the GLOBAL sums and count (backward); the count is read on the device, so ranks may hold different
  * batch sizes.  The parameter gradients (weight, bias, bn_weight, bn_bias, prelu) stay LOCAL sums, as in
@@ -215,25 +154,69 @@ typedef struct dgcn_bn_sync {
   void* user;
 } dgcn_bn_sync;
 
-/* dgcn_graph_conv_forward / dgcn_dyn_conv_forward / dgcn_graph_conv_backward with an optional dgcn_bn_sync.
- * sync == NULL, or a norm other than DGCN_NORM_BATCH_TRAIN: exactly the function without the suffix (same
- * results, bit for bit, and reduce is never called).  Same workspace sizes as the functions without it. */
-int dgcn_graph_conv_forward_sync(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N,
-                                 int64_t stride_b, int64_t stride_c, const int64_t* edge_index,
-                                 const int32_t* nbr, int64_t k, const dgcn_basic_conv* p,
-                                 int64_t C_out, float* out, const dgcn_bn_sync* sync, void* ws,
-                                 size_t ws_bytes, dgcn_stream_t stream);
-int dgcn_dyn_conv_forward_sync(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N,
-                               int64_t stride_b, int64_t stride_c, const dgcn_dilation* dil,
-                               const dgcn_basic_conv* p, int64_t C_out, float* out, int32_t* nbr_out,
-                               const dgcn_bn_sync* sync, void* ws, size_t ws_bytes, dgcn_stream_t stream);
-int dgcn_graph_conv_backward_sync(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N,
-                                  int64_t stride_b, int64_t stride_c, const int64_t* edge_index,
-                                  const int32_t* nbr, int64_t k,
-                                  const dgcn_basic_conv* p, int64_t C_out, const float* grad_out,
-                                  float* grad_x, float* grad_weight, float* grad_bias,
-                                  float* grad_bn_weight, float* grad_bn_bias, float* grad_prelu,
-                                  const dgcn_bn_sync* sync, void* ws, size_t ws_bytes, dgcn_stream_t stream);
+/* Static graph convolution on a given graph.
+ * Replaces gcn_lib/dense/torch_vertex.py:38-52 (GraphConv2d.forward) =
+ * EdgeConv2d.forward :31-35 / MRConv2d.forward :16-20, including
+ * batched_index_select (gcn_lib/dense/torch_nn.py:75-96) and BasicConv
+ * (torch_nn.py:48-58: conv1x1 -> act -> norm) and the max over neighbours.
+ * The graph comes either as the reference's int64 edge_index (2,B,N,k) with
+ * arbitrary centres, or as nbr (B,N,k) int32 with centre = own index.
+ * out: (B, C_out, N) contiguous.  sync: dgcn_bn_sync or NULL. */
+size_t dgcn_graph_conv_workspace_bytes(int32_t conv, int64_t B, int64_t C_in, int64_t C_out,
+                                       int64_t N, int64_t k);
+int dgcn_graph_conv_forward(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N,
+                            int64_t stride_b, int64_t stride_c, const int64_t* edge_index,
+                            const int32_t* nbr, int64_t k, const dgcn_basic_conv* p,
+                            int64_t C_out, float* out, const dgcn_bn_sync* sync /* may be NULL */,
+                            void* ws, size_t ws_bytes, dgcn_stream_t stream);
+
+/* Dynamic graph convolution: dilated kNN graph on x, then the convolution, in
+ * one call; the neighbour list goes from the selection kernel's shared memory
+ * straight into the gather/max and never reaches HBM unless nbr_out != NULL.
+ * Replaces gcn_lib/dense/torch_vertex.py:55-72 (DynConv2d.forward with
+ * knn='matrix').  fus: dgcn_block_fusion or NULL; sync: dgcn_bn_sync or NULL. */
+size_t dgcn_dyn_conv_workspace_bytes(int32_t conv, int64_t B, int64_t C_in, int64_t C_out,
+                                     int64_t N, int64_t K);
+
+/* Block epilogue around the dynamic convolution (SURVEY.md 8f rank 1), inference (no train-mode BatchNorm: with
+ * DGCN_NORM_BATCH_TRAIN a fusion returns DGCN_ERR_UNSUPPORTED):
+ *   residual != NULL: out = conv(x) + residual * res_scale   (ResDynBlock2d.forward, gcn_lib/dense/torch_vertex.py:101;
+ *     residual (B, C_out, N) with strides res_stride_b / res_stride_c, unit stride along points)
+ *   out_stride_b != 0: batch stride of `out` in floats - `out` is a channel slice of a wider (B, C_total, N) buffer
+ *     (DenseDynBlock2d's torch.cat, :116, or a model's fusion buffer, examples/sem_seg_dense/architecture.py:52). */
+typedef struct dgcn_block_fusion {
+  const float* residual;
+  int64_t res_stride_b, res_stride_c;
+  float res_scale;
+  int64_t out_stride_b;
+} dgcn_block_fusion;
+int dgcn_dyn_conv_forward(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N,
+                          int64_t stride_b, int64_t stride_c, const dgcn_dilation* dil,
+                          const dgcn_basic_conv* p, int64_t C_out, float* out, int32_t* nbr_out,
+                          const dgcn_block_fusion* fus /* may be NULL */,
+                          const dgcn_bn_sync* sync /* may be NULL */, void* ws, size_t ws_bytes,
+                          dgcn_stream_t stream);
+
+/* Gradient of dgcn_graph_conv_forward w.r.t. x and the BasicConv parameters
+ * (what torch autograd derives for torch_vertex.py:16-35 + torch_nn.py:48-58).
+ * The graph is the one used in forward (edge_index (2,B,N,k) int64 or nbr
+ * (B,N,k) int32 with centre = own index; the kNN graph itself is
+ * non-differentiable, torch_edge.py:53-56).  With DGCN_NORM_BATCH_TRAIN,
+ * p->bn_mean / p->bn_var must hold the BATCH statistics the forward returned.
+ * grad_x is (B, C_in, N) contiguous.
+ * grad_weight (C_out,2*C_in), grad_bias (C_out), grad_bn_weight/bias (C_out),
+ * grad_prelu (1) are OVERWRITTEN; any of them may be NULL.
+ * sync: dgcn_bn_sync or NULL. */
+size_t dgcn_graph_conv_backward_workspace_bytes(int32_t conv, int64_t B, int64_t C_in,
+                                                int64_t C_out, int64_t N, int64_t k);
+int dgcn_graph_conv_backward(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N,
+                             int64_t stride_b, int64_t stride_c, const int64_t* edge_index,
+                             const int32_t* nbr, int64_t k,
+                             const dgcn_basic_conv* p, int64_t C_out, const float* grad_out,
+                             float* grad_x, float* grad_weight, float* grad_bias,
+                             float* grad_bn_weight, float* grad_bn_bias, float* grad_prelu,
+                             const dgcn_bn_sync* sync /* may be NULL */, void* ws, size_t ws_bytes,
+                             dgcn_stream_t stream);
 
 /* ------------------------------------------------------------------------
  * Sparse path
@@ -264,16 +247,6 @@ typedef struct dgcn_genconv_params {
                                explicit messages, torch_message.py:44); 0: relu(.)+eps */
 } dgcn_genconv_params;
 
-/* Fused GENConv message + aggregate + MsgNorm + residual:
- *   msg_e = relu(x[src_e] + edge_attr[eid_e]) + eps     torch_vertex.py:78-85
- *   m_i   = aggregate_{e -> i}(msg_e)                   torch_message.py:44-85
- *   m_i   = scale * |x_i|_2 * m_i / max(|m_i|_2, 1e-12) torch_message.py:95-99
- *   out_i = x_i + m_i                                   torch_vertex.py:73
- * x_src (N_src, C) holds the rows that sources index (on one GPU the same array
- * as x_dst; under node partitioning local rows followed by halo rows);
- * x_dst (N, C) the rows of the destinations this call owns (may be NULL when neither
- * msg_norm nor add_residual is set).
- * edge_attr (E, C) in edge_index order or NULL.  out (N, C). */
 /* Long rows ("hubs" of power-law graphs): rows of in-degree >= min_degree are cut into segments of
  * seg_edges edges.  dgcn_csr_hub_rows lists them once per graph, entirely on the device:
  *   items  (2 * max_items int32): (row, segment) pairs, max_items = E / seg_edges + N_hub <= E/seg + E/min_degree + 1
@@ -292,12 +265,6 @@ typedef struct dgcn_csr_hubs {
 int dgcn_csr_hub_rows(const int32_t* rowptr, int64_t N, int64_t E, int32_t min_degree, int32_t seg_edges,
                       int32_t* items, int32_t* rows, int32_t* counts, dgcn_stream_t stream);
 
-int dgcn_genconv_aggregate(const float* x_src, const float* x_dst, int64_t N, int64_t C,
-                           const int32_t* rowptr, const int32_t* src, const int32_t* eid,
-                           const float* edge_attr, const dgcn_genconv_params* prm,
-                           const dgcn_csr_hubs* hubs /* may be NULL */, float* out,
-                           dgcn_stream_t stream);
-
 /* Block fusion around the aggregate (SURVEY.md 8f rank 1; DeeperGCN 'res+' block,
  * examples/ogb/ogbn_arxiv/model.py:91-106: h <- GENConv(relu(norm(h))) + h) and the split launch
  * that lets a node-partitioned layer overlap its halo exchange:
@@ -315,23 +282,6 @@ typedef struct dgcn_genconv_fusion {
   const int32_t* row_list;
   int64_t n_rows;
 } dgcn_genconv_fusion;
-int dgcn_genconv_aggregate_fused(const float* x_src, const float* x_dst, int64_t N, int64_t C,
-                                 const int32_t* rowptr, const int32_t* src, const int32_t* eid,
-                                 const float* edge_attr, const dgcn_genconv_params* prm,
-                                 const dgcn_csr_hubs* hubs /* may be NULL */,
-                                 const dgcn_genconv_fusion* fus /* may be NULL */, float* out,
-                                 dgcn_stream_t stream);
-/* The same on rows of element type `dtype` (dgcn_dtype; dgcn_genconv_aggregate_fused = DGCN_F32): x_src, x_dst and
- * edge_attr are all of that type, out stays fp32.  For DGCN_BF16 / DGCN_F16 the result is bit-identical to the
- * fp32 call on the same rows converted to fp32.  Half rows need C % 4 == 0, C <= 1024, 8-byte aligned x_src /
- * x_dst / edge_attr, a 16-byte aligned out and no pre-activation (fus->pre_scale NULL); anything else returns
- * DGCN_ERR_UNSUPPORTED. */
-int dgcn_genconv_aggregate_fused_rows(int32_t dtype, const void* x_src, const void* x_dst, int64_t N, int64_t C,
-                                      const int32_t* rowptr, const int32_t* src, const int32_t* eid,
-                                      const void* edge_attr, const dgcn_genconv_params* prm,
-                                      const dgcn_csr_hubs* hubs /* may be NULL */,
-                                      const dgcn_genconv_fusion* fus /* may be NULL */, float* out,
-                                      dgcn_stream_t stream);
 
 /* Dropout folded into the pre-activation of the res+ block in training (examples/ogb/ogbn_arxiv/model.py:91-106:
  * dropout(relu(norm(h)))).  keep_bits (N_src, words_per_row) int32 words, bit c % 32 of word c / 32 set when
@@ -344,16 +294,31 @@ typedef struct dgcn_keep_mask {
   int64_t words_per_row;
   float keep_scale;
 } dgcn_keep_mask;
-/* dgcn_genconv_aggregate_fused_rows plus a keep mask (NULL: exactly dgcn_genconv_aggregate_fused_rows).  A keep
- * mask needs fp32 rows, a pre-activation with pre_relu != 0 and no edge_attr; anything else returns
- * DGCN_ERR_UNSUPPORTED. */
-int dgcn_genconv_aggregate_fused_keep(int32_t dtype, const void* x_src, const void* x_dst, int64_t N, int64_t C,
-                                      const int32_t* rowptr, const int32_t* src, const int32_t* eid,
-                                      const void* edge_attr, const dgcn_genconv_params* prm,
-                                      const dgcn_csr_hubs* hubs /* may be NULL */,
-                                      const dgcn_genconv_fusion* fus /* may be NULL */,
-                                      const dgcn_keep_mask* keep /* may be NULL */, float* out,
-                                      dgcn_stream_t stream);
+
+/* Fused GENConv message + aggregate + MsgNorm + residual:
+ *   msg_e = relu(x[src_e] + edge_attr[eid_e]) + eps     torch_vertex.py:78-85
+ *   m_i   = aggregate_{e -> i}(msg_e)                   torch_message.py:44-85
+ *   m_i   = scale * |x_i|_2 * m_i / max(|m_i|_2, 1e-12) torch_message.py:95-99
+ *   out_i = x_i + m_i                                   torch_vertex.py:73
+ * x_src (N_src, C) holds the rows that sources index (on one GPU the same array
+ * as x_dst; under node partitioning local rows followed by halo rows);
+ * x_dst (N, C) the rows of the destinations this call owns (may be NULL when neither
+ * msg_norm nor add_residual is set).
+ * edge_attr (E, C) in edge_index order or NULL.  out (N, C).
+ * dtype (dgcn_dtype): x_src, x_dst and edge_attr are all of that type, out stays fp32.  For DGCN_BF16 / DGCN_F16
+ * the result is bit-identical to the fp32 call on the same rows converted to fp32.  Half rows need C % 4 == 0,
+ * C <= 1024, 8-byte aligned x_src / x_dst / edge_attr, a 16-byte aligned out and no pre-activation
+ * (fus->pre_scale NULL); anything else returns DGCN_ERR_UNSUPPORTED.
+ * hubs: dgcn_csr_hubs or NULL; fus: dgcn_genconv_fusion or NULL.
+ * keep: dgcn_keep_mask or NULL.  A keep mask needs fp32 rows, a pre-activation with pre_relu != 0 and no
+ * edge_attr; anything else returns DGCN_ERR_UNSUPPORTED. */
+int dgcn_genconv_aggregate(int32_t dtype, const void* x_src, const void* x_dst, int64_t N, int64_t C,
+                           const int32_t* rowptr, const int32_t* src, const int32_t* eid,
+                           const void* edge_attr, const dgcn_genconv_params* prm,
+                           const dgcn_csr_hubs* hubs /* may be NULL */,
+                           const dgcn_genconv_fusion* fus /* may be NULL */,
+                           const dgcn_keep_mask* keep /* may be NULL */, float* out,
+                           dgcn_stream_t stream);
 /* Bit-pack a keep mask: keep (N, C) fp32 (non-zero = kept, what Tensor.bernoulli_ draws) -> keep_bits
  * (N, ceil(C / 32)) int32 in the dgcn_keep_mask layout (bits of channels >= C are 0). */
 int dgcn_keep_bits_pack(const float* keep, int64_t N, int64_t C, int32_t* keep_bits, dgcn_stream_t stream);
@@ -377,40 +342,23 @@ int dgcn_linear_residual(const float* a, int64_t N, int64_t K, const float* weig
  * grad_x_src (N_src, C) must be zero-initialised by the caller (rows are
  * accumulated with atomics); grad_x_dst (N, C) is overwritten and may alias
  * nothing.  grad_scalars (4) = d/dt, d/dp, d/dy, d/dmsg_scale, accumulated with
- * atomics into a zero-initialised array; may be NULL. */
-int dgcn_genconv_aggregate_backward(const float* x_src, const float* x_dst, int64_t N,
+ * atomics into a zero-initialised array; may be NULL.
+ * dtype (dgcn_dtype): x_src, x_dst, edge_attr and grad_edge_attr are of that type; grad_out, grad_x_src,
+ * grad_x_dst and grad_scalars stay fp32.  For half rows grad_edge_attr is written once per CSR edge, rounded to
+ * nearest even (no zero-initialisation needed when eid covers every edge_attr row).  Half rows need C % 4 == 0.
+ * pre_scale / pre_shift (C) or both NULL, pre_relu: the forward's pre-activation (see dgcn_genconv_fusion); keep:
+ * its keep mask (dgcn_keep_mask) or NULL.  The rows are recomputed from x exactly as the forward read them, and
+ * grad_x_src / grad_x_dst are the gradients w.r.t. those activated rows (the caller applies the chain rule through
+ * the pre-activation).  A pre-activation needs fp32 rows; a keep mask needs a pre-activation with pre_relu != 0
+ * and no edge_attr; C > 512 is unsupported; anything else returns DGCN_ERR_UNSUPPORTED. */
+int dgcn_genconv_aggregate_backward(int32_t dtype, const void* x_src, const void* x_dst, int64_t N,
                                     int64_t N_src, int64_t C, const int32_t* rowptr,
                                     const int32_t* src, const int32_t* eid,
-                                    const float* edge_attr, const dgcn_genconv_params* prm,
-                                    int32_t softmax_grad, const float* grad_out,
-                                    float* grad_x_src, float* grad_x_dst, float* grad_edge_attr,
-                                    float* grad_scalars, dgcn_stream_t stream);
-/* The same on rows of element type `dtype` (dgcn_genconv_aggregate_backward = DGCN_F32): x_src, x_dst, edge_attr
- * and grad_edge_attr are of that type; grad_out, grad_x_src, grad_x_dst and grad_scalars stay fp32.
- * grad_edge_attr is written once per CSR edge, rounded to nearest even (no zero-initialisation needed when eid
- * covers every edge_attr row).  Half rows need C % 4 == 0 and C <= 512; anything else returns
- * DGCN_ERR_UNSUPPORTED. */
-int dgcn_genconv_aggregate_backward_rows(int32_t dtype, const void* x_src, const void* x_dst, int64_t N,
-                                         int64_t N_src, int64_t C, const int32_t* rowptr,
-                                         const int32_t* src, const int32_t* eid,
-                                         const void* edge_attr, const dgcn_genconv_params* prm,
-                                         int32_t softmax_grad, const float* grad_out,
-                                         float* grad_x_src, float* grad_x_dst, void* grad_edge_attr,
-                                         float* grad_scalars, dgcn_stream_t stream);
-/* The same with the forward's pre-activation (pre_scale / pre_shift (C) or both NULL, pre_relu; see
- * dgcn_genconv_fusion) and keep mask (dgcn_keep_mask, may be NULL): the rows are recomputed from x exactly as the
- * forward read them, and grad_x_src / grad_x_dst are the gradients w.r.t. those activated rows (the caller applies
- * the chain rule through the pre-activation).  Without both it is dgcn_genconv_aggregate_backward_rows.  A
- * pre-activation needs fp32 rows; a keep mask needs a pre-activation with pre_relu != 0 and no edge_attr; C > 512
- * is unsupported; anything else returns DGCN_ERR_UNSUPPORTED. */
-int dgcn_genconv_aggregate_backward_keep(int32_t dtype, const void* x_src, const void* x_dst, int64_t N,
-                                         int64_t N_src, int64_t C, const int32_t* rowptr,
-                                         const int32_t* src, const int32_t* eid,
-                                         const void* edge_attr, const dgcn_genconv_params* prm,
-                                         int32_t softmax_grad, const float* pre_scale, const float* pre_shift,
-                                         int32_t pre_relu, const dgcn_keep_mask* keep /* may be NULL */,
-                                         const float* grad_out, float* grad_x_src, float* grad_x_dst,
-                                         void* grad_edge_attr, float* grad_scalars, dgcn_stream_t stream);
+                                    const void* edge_attr, const dgcn_genconv_params* prm,
+                                    int32_t softmax_grad, const float* pre_scale, const float* pre_shift,
+                                    int32_t pre_relu, const dgcn_keep_mask* keep /* may be NULL */,
+                                    const float* grad_out, float* grad_x_src, float* grad_x_dst,
+                                    void* grad_edge_attr, float* grad_scalars, dgcn_stream_t stream);
 /* Backward epilogue of the fused res+ block in training: one pass over (N, C) rows
  *   g_y = (g_src + g_dst) * (keep ? keep_scale : 0) * [pre_scale * h + pre_shift > 0]      written over g_src,
  * the gradient w.r.t. the BatchNorm output (keep may be NULL: all kept, scale 1), and per channel
@@ -426,12 +374,10 @@ int dgcn_res_plus_backward_dh(const float* g_y, const float* h, int64_t N, int64
                               const float* d, const float* grad_skip, float* grad_h, dgcn_stream_t stream);
 
 /* Halo packing for node-partitioned graphs (new functionality; the reference
- * has no multi-GPU sparse path, SURVEY.md 3.4): out[r,:] = x[rows[r],:]. */
-int dgcn_gather_rows(const float* x, int64_t C, const int32_t* rows, int64_t R, float* out,
+ * has no multi-GPU sparse path, SURVEY.md 3.4): out[r,:] = x[rows[r],:].
+ * x and out are of element type `dtype` (dgcn_dtype); rows are copied as is. */
+int dgcn_gather_rows(int32_t dtype, const void* x, int64_t C, const int32_t* rows, int64_t R, void* out,
                      dgcn_stream_t stream);
-/* The same for rows of element type `dtype` (dgcn_dtype): x and out are of that type, rows are copied as is. */
-int dgcn_gather_rows_typed(int32_t dtype, const void* x, int64_t C, const int32_t* rows, int64_t R, void* out,
-                           dgcn_stream_t stream);
 
 /* ------------------------------------------------------------------------
  * Measurement hook (bench.py): when enabled, the dominant kernel of each path

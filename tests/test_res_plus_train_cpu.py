@@ -1,7 +1,6 @@
-"""The fused res+ block in training, host side (no GPU needed): the C ABI declarations of the keep-mask entry points
-against include/dgcn.h, the routing rule (which calls take the fused training path and which run the four lines),
-the keep-bit layout and the BatchNorm1d running-statistics bookkeeping against nn.BatchNorm1d itself."""
-import os
+"""The fused res+ block in training, host side (no GPU needed): the dgcn_keep_mask struct against include/dgcn.h, the
+routing rule (which calls take the fused training path and which run the four lines), the keep-bit layout and the
+BatchNorm1d running-statistics bookkeeping against nn.BatchNorm1d itself."""
 import re
 import types
 
@@ -12,59 +11,13 @@ from torch import nn
 from deep_gcns_torch_b200 import _native
 from deep_gcns_torch_b200.gcn_lib import sparse as S
 from deep_gcns_torch_b200.gcn_lib.sparse import fused
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _header():
-    with open(os.path.join(ROOT, "include", "dgcn.h")) as fh:
-        return fh.read()
-
-
-def _params(name):
-    m = re.search(r"int %s\(([^;]*)\);" % name, _header())
-    assert m, name
-    return [re.sub(r"\s+", " ", p.strip()) for p in re.sub(r"/\*.*?\*/", "", m.group(1)).split(",")]
-
-
-class _FakeLib:
-    class _Fn:
-        pass
-
-    def __getattr__(self, name):
-        fn = self._Fn()
-        object.__setattr__(self, name, fn)
-        return fn
+from test_abi_cpu import header
 
 
 def test_keep_mask_struct_matches_header():
-    m = re.search(r"typedef struct dgcn_keep_mask \{([^}]*)\}", _header())
+    m = re.search(r"typedef struct dgcn_keep_mask \{([^}]*)\}", header())
     fields = [f.split()[-1].lstrip("*") for f in m.group(1).split(";") if f.strip()]
     assert fields == [f[0] for f in _native.KeepMaskC._fields_]
-
-
-def test_keep_entry_points_extend_the_typed_ones():
-    lib = _FakeLib()
-    _native._declare(lib)
-    fwd, fwd_old = _params("dgcn_genconv_aggregate_fused_keep"), _params("dgcn_genconv_aggregate_fused_rows")
-    assert fwd == fwd_old[:-2] + ["const dgcn_keep_mask* keep"] + fwd_old[-2:]
-    a, b = lib.dgcn_genconv_aggregate_fused_keep, lib.dgcn_genconv_aggregate_fused_rows
-    assert a.restype is b.restype
-    assert list(a.argtypes) == list(b.argtypes[:-2]) + [ctypes_ptr(_native.KeepMaskC)] + list(b.argtypes[-2:])
-    bwd, bwd_old = _params("dgcn_genconv_aggregate_backward_keep"), _params("dgcn_genconv_aggregate_backward_rows")
-    pre = ["const float* pre_scale", "const float* pre_shift", "int32_t pre_relu", "const dgcn_keep_mask* keep"]
-    assert bwd == bwd_old[:12] + pre + bwd_old[12:]
-    a, b = lib.dgcn_genconv_aggregate_backward_keep, lib.dgcn_genconv_aggregate_backward_rows
-    assert a.restype is b.restype
-    assert list(a.argtypes) == (list(b.argtypes[:12]) + [b.argtypes[1], b.argtypes[1], _native.c_i32,
-                                                          ctypes_ptr(_native.KeepMaskC)] + list(b.argtypes[12:]))
-    for name in ("dgcn_keep_bits_pack", "dgcn_res_plus_backward_gy", "dgcn_res_plus_backward_dh"):
-        assert len(getattr(lib, name).argtypes) == len(_params(name)), name
-
-
-def ctypes_ptr(t):
-    import ctypes
-    return ctypes.POINTER(t)
 
 
 # ---- routing ------------------------------------------------------------------------------------------------------

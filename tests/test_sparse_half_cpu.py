@@ -1,62 +1,18 @@
-"""bf16 / fp16 rows in the sparse GENConv path, host side: the C ABI declarations of the typed entry points against
-include/dgcn.h, and the rule that decides which rows the kernels read as they are (no GPU needed)."""
-import os
+"""bf16 / fp16 rows in the sparse GENConv path, host side: the dgcn_dtype enum against include/dgcn.h, and the rule
+that decides which rows the kernels read as they are (no GPU needed)."""
 import re
 
 import pytest
 import torch
 
 from deep_gcns_torch_b200 import _native
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _header():
-    with open(os.path.join(ROOT, "include", "dgcn.h")) as fh:
-        return fh.read()
+from test_abi_cpu import header
 
 
 def test_dtype_enum_matches_header():
-    m = re.search(r"enum dgcn_dtype \{([^}]*)\}", _header())
+    m = re.search(r"enum dgcn_dtype \{([^}]*)\}", header())
     vals = dict((k.strip(), int(v)) for k, v in (e.split("=") for e in m.group(1).split(",")))
     assert vals == {"DGCN_F32": _native.DTYPE_F32, "DGCN_BF16": _native.DTYPE_BF16, "DGCN_F16": _native.DTYPE_F16}
-
-
-def _params(name):
-    m = re.search(r"int %s\(([^;]*)\);" % name, _header())
-    assert m, name
-    return [p.strip() for p in re.sub(r"/\*.*?\*/", "", m.group(1)).split(",")]
-
-
-class _FakeLib:
-    """Collects what _native._declare sets, so the declarations can be read without the built library."""
-
-    class _Fn:
-        pass
-
-    def __getattr__(self, name):
-        fn = self._Fn()
-        object.__setattr__(self, name, fn)
-        return fn
-
-
-@pytest.mark.parametrize("name,based_on", [
-    ("dgcn_genconv_aggregate_fused_rows", "dgcn_genconv_aggregate_fused"),
-    ("dgcn_genconv_aggregate_backward_rows", "dgcn_genconv_aggregate_backward"),
-    ("dgcn_gather_rows_typed", "dgcn_gather_rows"),
-])
-def test_typed_entry_points_are_the_fp32_ones_plus_a_leading_dtype(name, based_on):
-    new, old = _params(name), _params(based_on)
-    assert new[0] == "int32_t dtype"
-    assert len(new) == len(old) + 1
-    for a, b in zip(new[1:], old):      # same parameters; row pointers widened from float* to void*
-        assert a.split()[-1].lstrip("*") == b.split()[-1].lstrip("*")
-        assert a.replace("void*", "float*") == b or a == b, (a, b)
-    lib = _FakeLib()
-    _native._declare(lib)
-    fn, ref = getattr(lib, name), getattr(lib, based_on)
-    assert fn.restype is ref.restype
-    assert fn.argtypes[0] is _native.c_i32 and list(fn.argtypes[1:]) == list(ref.argtypes)
 
 
 def _rows(dtype, n=6, c=8):

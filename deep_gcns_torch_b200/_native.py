@@ -187,6 +187,16 @@ def _declare(lib):
     lib.dgcn_debug_tc_certification.argtypes = [c_i32]
     lib.dgcn_debug_tc_certification_read.restype = ctypes.c_int
     lib.dgcn_debug_tc_certification_read.argtypes = [ctypes.POINTER(c_i64), ctypes.POINTER(c_i64)]
+    lib.dgcn_sparse_edge_conv_workspace_bytes.restype = sz
+    lib.dgcn_sparse_edge_conv_workspace_bytes.argtypes = [c_i64] * 3
+    lib.dgcn_sparse_edge_conv_forward.restype = ctypes.c_int
+    lib.dgcn_sparse_edge_conv_forward.argtypes = [vp, c_i64, c_i64, vp, vp, c_i64, ctypes.POINTER(BasicConvC), c_i64,
+                                                  vp, vp, sz, vp]
+    lib.dgcn_sparse_edge_conv_backward_workspace_bytes.restype = sz
+    lib.dgcn_sparse_edge_conv_backward_workspace_bytes.argtypes = [c_i64] * 3
+    lib.dgcn_sparse_edge_conv_backward.restype = ctypes.c_int
+    lib.dgcn_sparse_edge_conv_backward.argtypes = [vp, c_i64, c_i64, vp, vp, c_i64, ctypes.POINTER(BasicConvC), c_i64,
+                                                   vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
     lib.dgcn_gather_rows.restype = ctypes.c_int
     lib.dgcn_gather_rows.argtypes = [c_i32, vp, c_i64, vp, c_i64, vp, vp]
     lib.dgcn_keep_bits_pack.restype = ctypes.c_int
@@ -507,6 +517,61 @@ def csr_build(edge_index, num_nodes):
                 hubs = (items, rows, counts, n_items)
     # (src / eid keep >= 1 element: a 0-element tensor has a null data_ptr)
     return rowptr, src, eid, hubs
+
+
+def _sparse_rows(x, csr):
+    """x (N, C_in) as the sparse EdgeConv reads it (fp32, contiguous) and the CSR's rowptr / src."""
+    rowptr, src = csr[0], csr[1]
+    _require_cuda(x, rowptr, src)
+    if x.dim() != 2 or x.dtype != torch.float32:
+        raise RuntimeError("sparse EdgeConv takes fp32 (N, C) node features, got %s %s" % (x.dtype, tuple(x.shape)))
+    return x.detach().contiguous(), rowptr, src
+
+
+def sparse_edge_conv_forward(x, csr, E, prm):
+    """dgcn_sparse_edge_conv_forward: out (N, C_out) over the CSR graph (csr_build) of E edges; in train mode
+    prm.batch_mean / prm.batch_var receive the batch statistics of the E edge rows."""
+    x, rowptr, src = _sparse_rows(x, csr)
+    _require_cuda(*prm.tensors())
+    N, C = x.shape
+    c_out = prm.weight.shape[0]
+    dev = x.device
+    with torch.cuda.device(dev):
+        l = lib()
+        cs = prm.c_struct(dev)
+        out = torch.empty((N, c_out), dtype=torch.float32, device=dev)
+        ws = _workspace(l.dgcn_sparse_edge_conv_workspace_bytes(N, C, c_out), dev)
+        rc = l.dgcn_sparse_edge_conv_forward(_ptr(x), N, C, _ptr(rowptr), _ptr(src), int(E), ctypes.byref(cs), c_out,
+                                             _ptr(out), _ptr(ws), ws.numel(), _stream(dev))
+        _check(rc, "dgcn_sparse_edge_conv_forward")
+    return out
+
+
+def sparse_edge_conv_backward(x, csr, E, prm, grad_out, need_x=True):
+    """dgcn_sparse_edge_conv_backward: dict of gradients (x, weight, bias, bn_weight, bn_bias, prelu)."""
+    x, rowptr, src = _sparse_rows(x, csr)
+    _require_cuda(grad_out)
+    N, C = x.shape
+    c_out = prm.weight.shape[0]
+    dev = x.device
+    go = _f32(grad_out)
+    with torch.cuda.device(dev):
+        l = lib()
+        stats = (prm.batch_mean, prm.batch_var) if prm.norm == NORM_BATCH_TRAIN else (prm.bn_mean, prm.bn_var)
+        cs = prm.c_struct(dev, stats)
+        f = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)
+        g = {"x": f(N, C) if need_x else None, "weight": f(c_out, 2 * C),
+             "bias": f(c_out) if prm.bias is not None else None,
+             "bn_weight": f(c_out) if prm.norm != NORM_NONE else None,
+             "bn_bias": f(c_out) if prm.norm != NORM_NONE else None,
+             "prelu": f(1) if prm.prelu_weight is not None else None}
+        ws = _workspace(l.dgcn_sparse_edge_conv_backward_workspace_bytes(N, C, c_out), dev)
+        rc = l.dgcn_sparse_edge_conv_backward(_ptr(x), N, C, _ptr(rowptr), _ptr(src), int(E), ctypes.byref(cs), c_out,
+                                              _ptr(go), _ptr(g["x"]), _ptr(g["weight"]), _ptr(g["bias"]),
+                                              _ptr(g["bn_weight"]), _ptr(g["bn_bias"]), _ptr(g["prelu"]), _ptr(ws),
+                                              ws.numel(), _stream(dev))
+        _check(rc, "dgcn_sparse_edge_conv_backward")
+    return g
 
 
 def _scalar(prm, name, value):

@@ -225,8 +225,7 @@ __global__ void __launch_bounds__(NTHREADS, 2)
 
 // Split-K "both operands k-contiguous" GEMM for weight gradients:
 //   out[r][c] += sum_{b, n in chunk} A[b][r][n] * Bm[b][c][n]      (atomicAdd, out zero-initialised)
-// one CTA = one 128x128 output tile x one chunk of KCH points of one cloud.
-constexpr int KCH = 512;
+// one CTA = one 128x128 output tile x one chunk of KCH points of one cloud (common.cuh).
 __global__ void __launch_bounds__(NTHREADS, 2)
     wgrad_kernel(const float* __restrict__ A, int64_t a_batch, int64_t lda, int rows, const float* __restrict__ Bm,
                  int64_t b_batch, int64_t ldb, int cols, int N, float* __restrict__ out, int64_t ldo) {

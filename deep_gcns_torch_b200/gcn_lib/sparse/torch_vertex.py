@@ -1,5 +1,6 @@
 """GENConv and the sparse-layout graph convolutions / blocks - API of the reference's
-gcn_lib/sparse/torch_vertex.py (GENConv :12-88; MRConv :91-103; GraphConv :239-266; DynConv :267-281; blocks :284-352)."""
+gcn_lib/sparse/torch_vertex.py (GENConv :12-88; MRConv :91-103; EdgConv :106-114; GraphConv :239-266; DynConv :267-281;
+blocks :284-352)."""
 import torch
 from torch import nn
 
@@ -8,7 +9,7 @@ from .torch_nn import MLP, BondEncoder
 from .torch_edge import DilatedKnnGraph
 from .torch_message import GenMessagePassing, MsgNorm, _AggregateFn, csr_of
 
-__all__ = ["GENConv", "MRConv", "GraphConv", "DynConv", "PlainDynBlock", "ResDynBlock", "DenseDynBlock",
+__all__ = ["GENConv", "MRConv", "EdgConv", "GraphConv", "DynConv", "PlainDynBlock", "ResDynBlock", "DenseDynBlock",
            "ResGraphBlock", "DenseGraphBlock"]
 
 
@@ -103,18 +104,118 @@ class MRConv(nn.Module):
         return self.nn(torch.cat([x, x_j], dim=1))
 
 
+class _EdgeConvFn(torch.autograd.Function):
+    """autograd node of EdgConv: dgcn_sparse_edge_conv_forward / _backward over the cached CSR graph."""
+
+    @staticmethod
+    def forward(ctx, owner, csr, n_edges, x, weight, bias, prelu, bn_w, bn_b):
+        prm = owner._conv_params()
+        out = _native.sparse_edge_conv_forward(x, csr, n_edges, prm)
+        owner._after_forward(prm, n_edges)
+        ctx.owner, ctx.prm, ctx.csr, ctx.n_edges = owner, prm, csr, n_edges
+        ctx.save_for_backward(x)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        (x,) = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        g = _native.sparse_edge_conv_backward(x, ctx.csr, ctx.n_edges, ctx.prm, grad_out, need_x=need[3])
+        pick = lambda i, key: g[key] if need[i] else None
+        return (None, None, None, pick(3, "x"), pick(4, "weight"), pick(5, "bias"), pick(6, "prelu"),
+                pick(7, "bn_weight"), pick(8, "bn_bias"))
+
+
+class EdgConv(nn.Module):
+    """Edge convolution, sparse layout (torch_vertex.py:106-114, torch_geometric's EdgeConv around
+    MLP([2*C_in, C_out], act, norm, bias): Linear -> norm -> act):
+    out_i = max over edges (j -> i) of nn(cat[x_i, x_j - x_i]), 0 for a node without in-edges.  One CSR edge pass
+    over the factorised Linear (z = P_i + Q_j, node-level GEMMs) keeps the max and min of z per node and channel;
+    the BatchNorm runs over the E edge rows.  Gradient of the max: the first edge in edge_index order that attains
+    it, as torch_scatter's scatter_max."""
+
+    def __init__(self, in_channels, out_channels, act="relu", norm=None, bias=True, aggr="max"):
+        super().__init__()
+        if aggr != "max":
+            raise NotImplementedError("EdgConv aggr {}: the sparse-layout EdgeConv aggregates with 'max'".format(aggr))
+        if norm is not None and str(norm).lower() not in ("none", "batch"):
+            raise NotImplementedError("EdgConv norm {}: the sparse-layout EdgeConv covers None and 'batch'".format(norm))
+        self.nn = MLP([in_channels * 2, out_channels], act, norm, bias)
+        self.aggr = aggr
+
+    def _parts(self):
+        lin, act, prelu, bn = self.nn[0], None, None, None
+        for m in list(self.nn)[1:]:
+            if isinstance(m, nn.ReLU):
+                act = "relu"
+            elif isinstance(m, nn.LeakyReLU):
+                act = "leakyrelu"
+            elif isinstance(m, nn.PReLU):
+                act, prelu = "prelu", m.weight
+            elif isinstance(m, nn.SyncBatchNorm):
+                raise NotImplementedError("EdgConv: SyncBatchNorm is not supported in the sparse-layout EdgeConv")
+            elif isinstance(m, nn.BatchNorm1d):
+                bn = m
+            else:
+                raise NotImplementedError("EdgConv: layer {} is not supported in the MLP".format(type(m).__name__))
+        if prelu is not None and prelu.numel() != 1:
+            raise NotImplementedError("EdgConv: PReLU with one weight per channel is not supported")
+        return lin, act, prelu, bn
+
+    def _conv_params(self):
+        lin, act, prelu, bn = self._parts()
+        norm, kw = _native.NORM_NONE, {}
+        if bn is not None:
+            use_batch = self.training or bn.running_mean is None
+            norm = _native.NORM_BATCH_TRAIN if use_batch else _native.NORM_BATCH_EVAL
+            kw = dict(bn_weight=bn.weight, bn_bias=bn.bias, bn_mean=bn.running_mean, bn_var=bn.running_var,
+                      bn_eps=bn.eps)
+        return _native.ConvParams(lin.weight, lin.bias, act, prelu, norm, **kw)
+
+    def _after_forward(self, prm, n_edges):
+        """BatchNorm1d training bookkeeping over the E edge rows, the rule of the dense convolutions' _after_forward
+        (momentum, unbiased variance, num_batches_tracked).  An edgeless batch leaves the running statistics as
+        torch does."""
+        bn = self._parts()[3]
+        if bn is None or prm.norm != _native.NORM_BATCH_TRAIN or not bn.track_running_stats:
+            return
+        with torch.no_grad():
+            bn.num_batches_tracked += 1
+            if n_edges == 0:
+                return
+            mom = bn.momentum if bn.momentum is not None else 1.0 / float(bn.num_batches_tracked)
+            unbiased = prm.batch_var * (n_edges / max(n_edges - 1, 1))
+            bn.running_mean.mul_(1 - mom).add_(prm.batch_mean, alpha=mom)
+            bn.running_var.mul_(1 - mom).add_(unbiased, alpha=mom)
+
+    def forward(self, x, edge_index):
+        lin, act, prelu, bn = self._parts()
+        _native._require_cuda(x, edge_index)
+        if x.dtype != torch.float32:
+            raise RuntimeError("EdgConv computes in fp32, got %s features" % x.dtype)
+        n_edges = int(edge_index.shape[1])
+        if bn is not None and (self.training or bn.running_mean is None) and n_edges == 1:
+            raise ValueError("Expected more than 1 value per channel when training, got input size %s"
+                             % (torch.Size([1, lin.out_features]),))       # what BatchNorm1d raises
+        csr = csr_of(edge_index, x.size(0))
+        return _EdgeConvFn.apply(self, csr, n_edges, x, lin.weight, lin.bias, prelu,
+                                 None if bn is None else bn.weight, None if bn is None else bn.bias)
+
+
 class GraphConv(nn.Module):
-    """Static graph convolution, sparse layout (torch_vertex.py:239-266).  'mr' runs on the CSR kernels; the other
-    variants are thin wrappers over third-party PyG convolutions in the reference (EdgeConv, GATConv, GCNConv,
-    GINConv, SAGEConv) and are not part of the rebuilt path - EdgeConv lives in gcn_lib.dense."""
+    """Static graph convolution, sparse layout (torch_vertex.py:239-266).  'edge' (EdgConv) and 'mr' (MRConv) run on
+    the CSR kernels; the other variants are thin wrappers over third-party PyG convolutions in the reference
+    (GATConv, GCNConv, GINConv, SAGEConv) and are not part of the rebuilt path."""
 
     def __init__(self, in_channels, out_channels, conv="edge", act="relu", norm=None, bias=True, heads=8):
         super().__init__()
-        if conv.lower() == "mr":
+        if conv.lower() == "edge":
+            self.gconv = EdgConv(in_channels, out_channels, act, norm, bias)
+        elif conv.lower() == "mr":
             self.gconv = MRConv(in_channels, out_channels, act, norm, bias)
-        elif conv.lower() in ("edge", "gat", "gcn", "gin", "sage", "rsage"):
+        elif conv.lower() in ("gat", "gcn", "gin", "sage", "rsage"):
             raise NotImplementedError("conv {}: a torch_geometric layer in the reference; the sparse-layout path here "
-                                      "covers 'mr' (EdgeConv: gcn_lib.dense)".format(conv))
+                                      "covers 'edge' and 'mr'".format(conv))
         else:
             raise NotImplementedError("conv {} is not implemented".format(conv))
 

@@ -373,6 +373,34 @@ int dgcn_res_plus_backward_gy(const float* h, int64_t N, int64_t C, const float*
 int dgcn_res_plus_backward_dh(const float* g_y, const float* h, int64_t N, int64_t C, const float* a, const float* b,
                               const float* d, const float* grad_skip, float* grad_h, dgcn_stream_t stream);
 
+/* EdgeConv in the sparse layout.
+ * Replaces gcn_lib/sparse/torch_vertex.py:106-114 (EdgConv = torch_geometric's EdgeConv with aggr 'max' around
+ * MLP([2*C_in, C_out], act, norm, bias), gcn_lib/sparse/torch_nn.py:50-68).  The order is Linear -> norm -> act
+ * (the dense BasicConv's is conv -> act -> norm):
+ *   out_i = max over edges e = (j -> i) of act(BN(W [x_i ; x_j - x_i] + b)),   out_i = 0 without in-edges;
+ * duplicate edges and self-loops count as ordinary edges.  With DGCN_NORM_BATCH_TRAIN the BatchNorm normalises
+ * with the statistics of the E edge rows (written to p->batch_mean_out / batch_var_out, biased variance).
+ * x (N, C_in) row-major fp32; the graph is dgcn_csr_build's rowptr (N+1) / src (E) of the edge_index (rows =
+ * targets, edges in edge_index order); p: the MLP's parameters in dgcn_basic_conv (weight = the Linear's
+ * (C_out, 2*C_in) weight, bn_* = the BatchNorm1d's); out (N, C_out) row-major fp32.
+ * N <= 65535 * 32; ws: dgcn_sparse_edge_conv_workspace_bytes(N, C_in, C_out). */
+size_t dgcn_sparse_edge_conv_workspace_bytes(int64_t N, int64_t C_in, int64_t C_out);
+int dgcn_sparse_edge_conv_forward(const float* x, int64_t N, int64_t C_in, const int32_t* rowptr,
+                                  const int32_t* src, int64_t E, const dgcn_basic_conv* p, int64_t C_out,
+                                  float* out, void* ws, size_t ws_bytes, dgcn_stream_t stream);
+/* Gradient of dgcn_sparse_edge_conv_forward w.r.t. x and the MLP's parameters (what torch autograd derives for the
+ * reference, with the max's gradient going to the first edge in edge_index order that attains it, per node and
+ * channel, as torch_scatter's scatter_max).  With DGCN_NORM_BATCH_TRAIN, p->bn_mean / p->bn_var must hold the
+ * BATCH statistics the forward returned.  grad_x (N, C_in), grad_weight (C_out, 2*C_in), grad_bias (C_out),
+ * grad_bn_weight / grad_bn_bias (C_out), grad_prelu (1) are OVERWRITTEN; any of them may be NULL.
+ * ws: dgcn_sparse_edge_conv_backward_workspace_bytes(N, C_in, C_out). */
+size_t dgcn_sparse_edge_conv_backward_workspace_bytes(int64_t N, int64_t C_in, int64_t C_out);
+int dgcn_sparse_edge_conv_backward(const float* x, int64_t N, int64_t C_in, const int32_t* rowptr,
+                                   const int32_t* src, int64_t E, const dgcn_basic_conv* p, int64_t C_out,
+                                   const float* grad_out, float* grad_x, float* grad_weight, float* grad_bias,
+                                   float* grad_bn_weight, float* grad_bn_bias, float* grad_prelu, void* ws,
+                                   size_t ws_bytes, dgcn_stream_t stream);
+
 /* Halo packing for node-partitioned graphs (new functionality; the reference
  * has no multi-GPU sparse path, SURVEY.md 3.4): out[r,:] = x[rows[r],:].
  * x and out are of element type `dtype` (dgcn_dtype); rows are copied as is. */

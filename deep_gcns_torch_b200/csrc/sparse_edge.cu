@@ -100,7 +100,7 @@ __global__ void __launch_bounds__(SPE_WARPS * 32) sp_edge_fwd_kernel(const SpEdg
     const bool live = c < co;
     float s = 1.f, t = 0.f, mean, inv;
     if (!TRAIN) sp_edge_affine(g, c, s, t, mean, inv);   // (train mode: the statistics come from this pass)
-    BnAcc st = bn_acc_zero();
+    BnMoments st{0.f, 0.f, 0.f};
     for (int u = 0; u < SPE_ROWS_PER_WARP; ++u) {
       const int i = blockIdx.x * SPE_ROWS + warp * SPE_ROWS_PER_WARP + u;
       if (i >= g.N) break;
@@ -110,14 +110,18 @@ __global__ void __launch_bounds__(SPE_WARPS * 32) sp_edge_fwd_kernel(const SpEdg
       for (int e0 = beg; e0 < end; e0 += 32) {
         const int mine = e0 + lane < end ? __ldg(g.src + e0 + lane) : 0;
         const int n = min(32, end - e0);
+        BnAcc acc = bn_acc_zero();
         for (int q = 0; q < n; ++q) {
           const int j = __shfl_sync(0xffffffffu, mine, q);
           if (!live) continue;
           const float z = p + __ldg(g.pq + static_cast<int64_t>(j) * ld + co + c);
           zmax = fmaxf(zmax, z);
           zmin = fminf(zmin, z);
-          if (TRAIN) bn_acc_add(st, z);
+          if (TRAIN) bn_acc_add(acc, z);
         }
+        // each 32-edge chunk is summed about its own first z and merged by Chan's formula: one running sum over a
+        // long row (or over rows of different P_i) would hold the squares of all its deviations from one pivot
+        if (TRAIN) st = bn_merge(st, bn_acc_moments(acc));
       }
       if (!live) continue;
       const int64_t o = static_cast<int64_t>(i) * co + c;
@@ -129,7 +133,7 @@ __global__ void __launch_bounds__(SPE_WARPS * 32) sp_edge_fwd_kernel(const SpEdg
       }
     }
     if (TRAIN) {
-      red[warp][lane] = bn_acc_moments(st);
+      red[warp][lane] = st;
       __syncthreads();
       if (warp == 0) {
         BnMoments m = red[0][lane];

@@ -125,11 +125,7 @@ def _assert_stats(mean, var, a64, const_channel=True, what=""):
 
 
 def _kernel_names(fn):
-    from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        res = fn()
-        torch.cuda.synchronize()
-    return res, {e.key for e in prof.key_averages()}
+    return bu.kernel_names(fn)
 
 
 # name: conv, kind (static edge_index / static nbr / dyn), knn path, B, C, N, k, dilation, c_out, act, writer kernel

@@ -26,11 +26,7 @@ KINDS = ["pad1", "pad25", "pad60", "zeros", "dup3"]
 
 
 def _kernel_names(fn):
-    from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        res = fn()
-        torch.cuda.synchronize()
-    return res, {e.key for e in prof.key_averages()}
+    return bu.kernel_names(fn)
 
 
 def _on_path(path, fn):

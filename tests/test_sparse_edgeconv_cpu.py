@@ -127,3 +127,43 @@ def test_unsupported_configurations_raise():
         S.EdgConv(4, 8)(x, ei)
     with pytest.raises(RuntimeError, match="CUDA"):
         S.GraphConv(4, 8, "edge")(x.double(), ei)
+
+
+@pytest.mark.parametrize("name", list(seu.EXACT_SHAPES))
+def test_exact_fixture_premises(name):
+    """The premises of tests/test_sparse_edgeconv_shapes_gpu.py's exact grid, for every fixture it builds: fp32 z from
+    the kernel's factorised form P_i + Q_j, with P and Q each summed in two orders (one channel at a time ascending,
+    and in chunks of 32 descending), is bit-equal to fp64 z of the reference's W [x_i; x_j - x_i] + b; in eval (eps = 0) so is
+    u = s z + t; the offset channels are un-centred (|mean| / std of z > 100 on the last channel); and in train mode
+    no fp64 top-two gap of distinct z, nor a winning |u|, is within edge_tie_mask's near-tie / kink bounds."""
+    N, ci, co, hub, seed = seu.EXACT_SHAPES[name]
+    acts = seu.ALL_ACTS if name in seu.BIG_SHAPES else seu.ALL_ACTS[:1]
+    for act, slope in acts:
+        for train in (False, True):
+            mod, x, ei, _ = seu.exact_fixture(N, ci, co, act, slope, train, seed, hub)
+            w, b = mod.nn[0].weight.detach(), mod.nn[0].bias.detach()
+            src, dst = ei[0], ei[1]
+            z64 = torch.nn.functional.linear(torch.cat([x[dst], x[src] - x[dst]], 1).double(), w.double(), b.double())
+            assert z64.abs().max() < 2.0 ** 20
+            w1, w2 = w[:, :ci], w[:, ci:]
+            for order, chunk in ((torch.arange(ci), 1), (torch.arange(ci).flip(0), 32)):
+                P = b.expand(N, co).clone()
+                Q = torch.zeros(N, co)
+                for c0 in range(0, ci, chunk):
+                    cs = order[c0:c0 + chunk]
+                    P += x[:, cs] @ (w1 - w2)[:, cs].T
+                    Q += x[:, cs] @ w2[:, cs].T
+                assert torch.equal((P[dst] + Q[src]).double(), z64), (name, act, train)
+            bn = mod.nn[1]
+            if not train:
+                s = bn.weight.detach() / torch.sqrt(bn.running_var + bn.eps)
+                t = bn.bias.detach() - bn.running_mean * s
+                z32 = z64.float()
+                assert torch.equal((s * z32 + t).double(), s.double() * z64 + t.double())
+            else:
+                if co >= 3:
+                    zc = z64[:, co - 1]
+                    assert float(zc.mean().abs() / zc.std()) > 100
+                assert int(seu.edge_tie_mask(mod.nn, x, ei, 1e-4, 1e-5, True, exact=True).sum()) == 0, (name, act)
+                if co >= 2:
+                    assert bool((z64[:, 1] == 0).all())

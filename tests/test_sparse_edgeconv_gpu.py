@@ -143,7 +143,7 @@ def test_gradients_against_fp64(training):
         mod.train(training)
         mask = seu.edge_tie_mask(mod.nn, x, ei, TIE_REL, KINK_REL, training)
         assert mask.double().mean() <= MAX_MASKED, (name, float(mask.double().mean()))
-        gout = torch.randn(c.meta["N"], c.meta["out"], generator=g).masked_fill(mask, 0.0)
+        gout = torch.randn(c.meta["N"], c.meta["out"], generator=g).masked_fill(mask.cpu(), 0.0)
         ref_y, ref = _oracle_grads(mod, act, x, ei, training, gout)
         y, got = _kernel_grads(mod, x, ei, gout)
         torch.testing.assert_close(y.cpu().double(), ref_y, rtol=RTOL, atol=ATOL)

@@ -191,12 +191,12 @@ def _declare(lib):
     lib.dgcn_sparse_edge_conv_workspace_bytes.argtypes = [c_i64] * 3
     lib.dgcn_sparse_edge_conv_forward.restype = ctypes.c_int
     lib.dgcn_sparse_edge_conv_forward.argtypes = [vp, c_i64, c_i64, vp, vp, c_i64, ctypes.POINTER(BasicConvC), c_i64,
-                                                  vp, vp, sz, vp]
+                                                  vp, ctypes.POINTER(BnSyncC), vp, sz, vp]
     lib.dgcn_sparse_edge_conv_backward_workspace_bytes.restype = sz
     lib.dgcn_sparse_edge_conv_backward_workspace_bytes.argtypes = [c_i64] * 3
     lib.dgcn_sparse_edge_conv_backward.restype = ctypes.c_int
     lib.dgcn_sparse_edge_conv_backward.argtypes = [vp, c_i64, c_i64, vp, vp, c_i64, ctypes.POINTER(BasicConvC), c_i64,
-                                                   vp, vp, vp, vp, vp, vp, vp, vp, sz, vp]
+                                                   vp, vp, vp, vp, vp, vp, vp, ctypes.POINTER(BnSyncC), vp, sz, vp]
     lib.dgcn_gather_rows.restype = ctypes.c_int
     lib.dgcn_gather_rows.argtypes = [c_i32, vp, c_i64, vp, c_i64, vp, vp]
     lib.dgcn_keep_bits_pack.restype = ctypes.c_int
@@ -530,7 +530,8 @@ def _sparse_rows(x, csr):
 
 def sparse_edge_conv_forward(x, csr, E, prm):
     """dgcn_sparse_edge_conv_forward: out (N, C_out) over the CSR graph (csr_build) of E edges; in train mode
-    prm.batch_mean / prm.batch_var receive the batch statistics of the E edge rows."""
+    prm.batch_mean / prm.batch_var receive the batch statistics of the E edge rows (with prm.sync_group, of every
+    rank's edge rows, and prm.moments their cross-rank moments)."""
     x, rowptr, src = _sparse_rows(x, csr)
     _require_cuda(*prm.tensors())
     N, C = x.shape
@@ -541,9 +542,13 @@ def sparse_edge_conv_forward(x, csr, E, prm):
         cs = prm.c_struct(dev)
         out = torch.empty((N, c_out), dtype=torch.float32, device=dev)
         ws = _workspace(l.dgcn_sparse_edge_conv_workspace_bytes(N, C, c_out), dev)
+        bs = prm.bn_sync(dev)
         rc = l.dgcn_sparse_edge_conv_forward(_ptr(x), N, C, _ptr(rowptr), _ptr(src), int(E), ctypes.byref(cs), c_out,
-                                             _ptr(out), _ptr(ws), ws.numel(), _stream(dev))
-        _check(rc, "dgcn_sparse_edge_conv_forward")
+                                             _ptr(out), None if bs is None else ctypes.byref(bs.c), _ptr(ws),
+                                             ws.numel(), _stream(dev))
+        (_check if bs is None else bs.check)(rc, "dgcn_sparse_edge_conv_forward")
+        if bs is not None:
+            prm.moments = bs.moments
     return out
 
 
@@ -566,11 +571,14 @@ def sparse_edge_conv_backward(x, csr, E, prm, grad_out, need_x=True):
              "bn_bias": f(c_out) if prm.norm != NORM_NONE else None,
              "prelu": f(1) if prm.prelu_weight is not None else None}
         ws = _workspace(l.dgcn_sparse_edge_conv_backward_workspace_bytes(N, C, c_out), dev)
+        bs = prm.bn_sync(dev)
+        # synced: dx from the cross-rank sums; the parameter gradients stay local (SyncBatchNorm)
         rc = l.dgcn_sparse_edge_conv_backward(_ptr(x), N, C, _ptr(rowptr), _ptr(src), int(E), ctypes.byref(cs), c_out,
                                               _ptr(go), _ptr(g["x"]), _ptr(g["weight"]), _ptr(g["bias"]),
-                                              _ptr(g["bn_weight"]), _ptr(g["bn_bias"]), _ptr(g["prelu"]), _ptr(ws),
-                                              ws.numel(), _stream(dev))
-        _check(rc, "dgcn_sparse_edge_conv_backward")
+                                              _ptr(g["bn_weight"]), _ptr(g["bn_bias"]), _ptr(g["prelu"]),
+                                              None if bs is None else ctypes.byref(bs.c), _ptr(ws), ws.numel(),
+                                              _stream(dev))
+        (_check if bs is None else bs.check)(rc, "dgcn_sparse_edge_conv_backward")
     return g
 
 

@@ -637,9 +637,9 @@ __global__ void bn_finalize_moments_kernel(const double* __restrict__ moments, i
 }
 
 // Train mode: (scale, shift) into st from the partial rows of `count` positions; with sync, from the
-// statistics of every rank.
-static int bn_finalize(const float* partial, int64_t np, int64_t co, double count, const dgcn_basic_conv* p,
-                       const dgcn_bn_sync* sync, float* st, cudaStream_t stream) {
+// statistics of every rank.  Shared with the sparse EdgeConv (sparse_edge.cu).
+int bn_finalize(const float* partial, int64_t np, int64_t co, double count, const dgcn_basic_conv* p,
+                const dgcn_bn_sync* sync, float* st, cudaStream_t stream) {
   const int C = static_cast<int>(co);
   bn_merge_kernel<<<static_cast<unsigned>(co), 256, 0, stream>>>(partial, np, C, count, p->bn_weight, p->bn_bias,
                                                                  p->bn_eps, st, p->batch_mean_out, p->batch_var_out,

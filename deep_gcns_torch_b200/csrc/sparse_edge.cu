@@ -17,6 +17,10 @@
 // BatchNorm backward (two passes: pass 0 forms sum du and sum du * zhat, pass 1 dz for every edge).  dP_i sums over
 // row i's edges in registers, dQ_j is accumulated with atomics, both into node-major dPQ; the parameter gradients and
 // grad_x are node-level products of dPQ.
+//
+// Synced statistics (dgcn_bn_sync, nn.SyncBatchNorm): the forward all-reduces this rank's moments of z between the
+// edge pass and the (s, t) finalisation (dense_fwd.cu's bn_finalize); the backward all-reduces pass 0's sums, and
+// pass 1 runs with the global sums over the global count.  The edge kernels are the same on both paths.
 #include "common.cuh"
 
 namespace dgcn {
@@ -30,12 +34,13 @@ __global__ void to_node_major_kernel(const float* __restrict__ x, int64_t sb, in
 __global__ void node_pq_kernel(const float* __restrict__ x, int64_t sb, int64_t sc, int C, int N, int vec,
                                const float* __restrict__ wk, const float* __restrict__ bk, int M,
                                float* __restrict__ pq);
-__global__ void bn_merge_kernel(const float* __restrict__ partial, int64_t np, int C, double count,
-                                const float* __restrict__ bn_w, const float* __restrict__ bn_b, float eps,
-                                float* __restrict__ st, float* __restrict__ mean_out, float* __restrict__ var_out,
-                                double* __restrict__ moments);
 __global__ void reduce_partials_kernel(const float* __restrict__ partial, int64_t np, int nq, int C,
                                        double* __restrict__ sums);
+int bn_finalize(const float* partial, int64_t np, int64_t co, double count, const dgcn_basic_conv* p,
+                const dgcn_bn_sync* sync, float* st, cudaStream_t stream);
+int bn_sync_moments(const float* partial, int64_t np, int nq, int C, double count, const dgcn_bn_sync* sync,
+                    cudaStream_t stream);
+__global__ void moments_over_count_kernel(const double* __restrict__ moments, int C, double* __restrict__ sums);
 __global__ void finish_param_grads_kernel(const double* __restrict__ sums, int C, int have_slope,
                                           float* __restrict__ grad_bn_w, float* __restrict__ grad_bn_b,
                                           float* __restrict__ grad_prelu);
@@ -290,8 +295,9 @@ static SpEdgeRegions carve_sp_edge(bool backward, int64_t N, int64_t ci, int64_t
 }
 
 static int check_sp_edge_args(const float* x, int64_t N, int64_t ci, const int32_t* rowptr, const int32_t* src,
-                              int64_t E, const dgcn_basic_conv* p, int64_t co) {
+                              int64_t E, const dgcn_basic_conv* p, int64_t co, const dgcn_bn_sync* sync) {
   if (!x || !rowptr || !src || !p || !p->weight || N <= 0 || ci <= 0 || co <= 0 || E < 0) return DGCN_ERR_BAD_ARG;
+  if (sync && (!sync->moments || !sync->reduce)) return DGCN_ERR_BAD_ARG;
   if (p->act < DGCN_ACT_NONE || p->act > DGCN_ACT_PRELU) return DGCN_ERR_UNSUPPORTED;
   if (p->act == DGCN_ACT_PRELU && !p->prelu_weight) return DGCN_ERR_BAD_ARG;
   if (p->norm < DGCN_NORM_NONE || p->norm > DGCN_NORM_BATCH_TRAIN) return DGCN_ERR_UNSUPPORTED;
@@ -343,9 +349,9 @@ size_t dgcn_sparse_edge_conv_workspace_bytes(int64_t N, int64_t C_in, int64_t C_
 }
 
 int dgcn_sparse_edge_conv_forward(const float* x, int64_t N, int64_t C_in, const int32_t* rowptr, const int32_t* src,
-                                  int64_t E, const dgcn_basic_conv* p, int64_t C_out, float* out, void* wsp,
-                                  size_t ws_bytes, dgcn_stream_t stream_) {
-  int rc = check_sp_edge_args(x, N, C_in, rowptr, src, E, p, C_out);
+                                  int64_t E, const dgcn_basic_conv* p, int64_t C_out, float* out,
+                                  const dgcn_bn_sync* sync, void* wsp, size_t ws_bytes, dgcn_stream_t stream_) {
+  int rc = check_sp_edge_args(x, N, C_in, rowptr, src, E, p, C_out, sync);
   if (rc != DGCN_OK) return rc;
   if (!out) return DGCN_ERR_BAD_ARG;
   if (p->norm == DGCN_NORM_BATCH_EVAL && (!p->bn_mean || !p->bn_var)) return DGCN_ERR_BAD_ARG;
@@ -368,11 +374,10 @@ int dgcn_sparse_edge_conv_forward(const float* x, int64_t N, int64_t C_in, const
   g.zmax = w.zmax; g.zmin = w.zmin; g.partial = w.partial;
   sp_edge_fwd_kernel<1><<<grid, SPE_WARPS * 32, 0, stream>>>(g);
   DGCN_LAUNCH_CHECK();
-  // batch statistics of z over the E edges -> (s, t), batch mean and biased variance
-  bn_merge_kernel<<<static_cast<unsigned>(C_out), 256, 0, stream>>>(
-      w.partial, sp_edge_ctas(N), static_cast<int>(C_out), static_cast<double>(E), p->bn_weight, p->bn_bias,
-      p->bn_eps, w.st, p->batch_mean_out, p->batch_var_out, nullptr);
-  DGCN_LAUNCH_CHECK();
+  // batch statistics of z over the E edges (with sync, over every rank's edges) -> (s, t), batch mean and biased
+  // variance; a rank without edges contributes count 0 and still makes its reduce call
+  rc = bn_finalize(w.partial, sp_edge_ctas(N), C_out, static_cast<double>(E), p, sync, w.st, stream);
+  if (rc != DGCN_OK) return rc;
   sp_edge_apply_kernel<<<static_cast<unsigned>(ceil_div(N * C_out, 256)), 256, 0, stream>>>(g, w.st);
   DGCN_LAUNCH_CHECK();
   return DGCN_OK;
@@ -387,9 +392,9 @@ size_t dgcn_sparse_edge_conv_backward_workspace_bytes(int64_t N, int64_t C_in, i
 int dgcn_sparse_edge_conv_backward(const float* x, int64_t N, int64_t C_in, const int32_t* rowptr,
                                    const int32_t* src, int64_t E, const dgcn_basic_conv* p, int64_t C_out,
                                    const float* grad_out, float* grad_x, float* grad_weight, float* grad_bias,
-                                   float* grad_bn_weight, float* grad_bn_bias, float* grad_prelu, void* wsp,
-                                   size_t ws_bytes, dgcn_stream_t stream_) {
-  int rc = check_sp_edge_args(x, N, C_in, rowptr, src, E, p, C_out);
+                                   float* grad_bn_weight, float* grad_bn_bias, float* grad_prelu,
+                                   const dgcn_bn_sync* sync, void* wsp, size_t ws_bytes, dgcn_stream_t stream_) {
+  int rc = check_sp_edge_args(x, N, C_in, rowptr, src, E, p, C_out, sync);
   if (rc != DGCN_OK) return rc;
   if (!grad_out) return DGCN_ERR_BAD_ARG;
   if (p->norm != DGCN_NORM_NONE && (!p->bn_mean || !p->bn_var)) return DGCN_ERR_BAD_ARG;
@@ -415,8 +420,21 @@ int dgcn_sparse_edge_conv_backward(const float* x, int64_t N, int64_t C_in, cons
     DGCN_LAUNCH_CHECK();
     reduce_partials_kernel<<<dim3(ico, 3), 256, 0, stream>>>(w.partial, n_cta, 3, ico, w.sums);
     DGCN_LAUNCH_CHECK();
+    // w.sums keeps this rank's sums: the parameter gradients are local, as in nn.SyncBatchNorm.  With sync, pass 1
+    // takes the global sums over the global count, divided in place in sync->moments (each entry is read and
+    // written by its own thread, the count at [2 co] by none), with inv_count = 1
+    const double* pass1 = w.sums;
+    if (sync) {
+      rc = bn_sync_moments(w.partial, n_cta, 3, ico, static_cast<double>(E), sync, stream);
+      if (rc != DGCN_OK) return rc;
+      moments_over_count_kernel<<<static_cast<unsigned>(ceil_div(2 * C_out, 128)), 128, 0, stream>>>(
+          sync->moments, ico, sync->moments);
+      DGCN_LAUNCH_CHECK();
+      pass1 = sync->moments;
+      g.inv_count = 1.0;
+    }
     // pass 1 wants (sum du, sum du * zhat) as float[2][co]: finish_param_grads_kernel does the conversion
-    finish_param_grads_kernel<<<static_cast<unsigned>(ceil_div(C_out, 128)), 128, 0, stream>>>(w.sums, ico, 0,
+    finish_param_grads_kernel<<<static_cast<unsigned>(ceil_div(C_out, 128)), 128, 0, stream>>>(pass1, ico, 0,
                                                                                                 w.sf + C_out, w.sf,
                                                                                                 nullptr);
     DGCN_LAUNCH_CHECK();

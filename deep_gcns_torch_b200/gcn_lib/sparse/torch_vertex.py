@@ -132,7 +132,8 @@ class EdgConv(nn.Module):
     out_i = max over edges (j -> i) of nn(cat[x_i, x_j - x_i]), 0 for a node without in-edges.  One CSR edge pass
     over the factorised Linear (z = P_i + Q_j, node-level GEMMs) keeps the max and min of z per node and channel;
     the BatchNorm runs over the E edge rows.  Gradient of the max: the first edge in edge_index order that attains
-    it, as torch_scatter's scatter_max."""
+    it, as torch_scatter's scatter_max.  After nn.SyncBatchNorm.convert_sync_batchnorm, train-mode statistics are those
+    of the edge rows of every rank in the BatchNorm's process group; the parameter gradients stay local."""
 
     def __init__(self, in_channels, out_channels, act="relu", norm=None, bias=True, aggr="max"):
         super().__init__()
@@ -152,9 +153,7 @@ class EdgConv(nn.Module):
                 act = "leakyrelu"
             elif isinstance(m, nn.PReLU):
                 act, prelu = "prelu", m.weight
-            elif isinstance(m, nn.SyncBatchNorm):
-                raise NotImplementedError("EdgConv: SyncBatchNorm is not supported in the sparse-layout EdgeConv")
-            elif isinstance(m, nn.BatchNorm1d):
+            elif isinstance(m, (nn.BatchNorm1d, nn.SyncBatchNorm)):
                 bn = m
             else:
                 raise NotImplementedError("EdgConv: layer {} is not supported in the MLP".format(type(m).__name__))
@@ -169,32 +168,41 @@ class EdgConv(nn.Module):
             use_batch = self.training or bn.running_mean is None
             norm = _native.NORM_BATCH_TRAIN if use_batch else _native.NORM_BATCH_EVAL
             kw = dict(bn_weight=bn.weight, bn_bias=bn.bias, bn_mean=bn.running_mean, bn_var=bn.running_var,
-                      bn_eps=bn.eps)
+                      bn_eps=bn.eps, sync_group=_native.sync_group(bn))
         return _native.ConvParams(lin.weight, lin.bias, act, prelu, norm, **kw)
 
     def _after_forward(self, prm, n_edges):
         """BatchNorm1d training bookkeeping over the E edge rows, the rule of the dense convolutions' _after_forward
         (momentum, unbiased variance, num_batches_tracked).  An edgeless batch leaves the running statistics as
-        torch does."""
+        torch does.  With synced statistics the variance is unbiased with the global edge count, read on the device,
+        and a rank without edges updates its running statistics from the global ones like its peers."""
         bn = self._parts()[3]
         if bn is None or prm.norm != _native.NORM_BATCH_TRAIN or not bn.track_running_stats:
             return
         with torch.no_grad():
             bn.num_batches_tracked += 1
-            if n_edges == 0:
+            if prm.moments is None and n_edges == 0:
                 return
             mom = bn.momentum if bn.momentum is not None else 1.0 / float(bn.num_batches_tracked)
-            unbiased = prm.batch_var * (n_edges / max(n_edges - 1, 1))
+            if prm.moments is not None:
+                count = prm.moments[-1]
+                unbiased = prm.batch_var * (count / (count - 1).clamp_min(1)).float()
+            else:
+                unbiased = prm.batch_var * (n_edges / max(n_edges - 1, 1))
             bn.running_mean.mul_(1 - mom).add_(prm.batch_mean, alpha=mom)
             bn.running_var.mul_(1 - mom).add_(unbiased, alpha=mom)
 
     def forward(self, x, edge_index):
         lin, act, prelu, bn = self._parts()
+        if isinstance(bn, nn.SyncBatchNorm) and not (x.is_cuda and edge_index.is_cuda):
+            raise NotImplementedError("EdgConv: the sparse EdgeConv's SyncBatchNorm needs CUDA tensors")
         _native._require_cuda(x, edge_index)
         if x.dtype != torch.float32:
             raise RuntimeError("EdgConv computes in fp32, got %s features" % x.dtype)
         n_edges = int(edge_index.shape[1])
-        if bn is not None and (self.training or bn.running_mean is None) and n_edges == 1:
+        # one edge row has no batch variance unless other ranks share the statistics (SyncBatchNorm's rule)
+        if bn is not None and (self.training or bn.running_mean is None) and n_edges == 1 and \
+                _native.sync_group(bn) is None:
             raise ValueError("Expected more than 1 value per channel when training, got input size %s"
                              % (torch.Size([1, lin.out_features]),))       # what BatchNorm1d raises
         csr = csr_of(edge_index, x.size(0))

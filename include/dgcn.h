@@ -131,12 +131,14 @@ int dgcn_knn_graph(const float* x, int64_t B, int64_t C, int64_t N, int64_t stri
                    dgcn_stream_t stream);
 
 /* Train-mode BatchNorm statistics shared across data-parallel ranks (torch.nn.SyncBatchNorm), the `sync`
- * argument of dgcn_graph_conv_forward, dgcn_dyn_conv_forward and dgcn_graph_conv_backward.  sync == NULL, or a
- * norm other than DGCN_NORM_BATCH_TRAIN: the statistics are the call's own (reduce is never called).  The
- * workspace sizes do not depend on it.
+ * argument of dgcn_graph_conv_forward, dgcn_dyn_conv_forward, dgcn_graph_conv_backward and
+ * dgcn_sparse_edge_conv_forward / _backward.  sync == NULL, or a norm other than DGCN_NORM_BATCH_TRAIN: the
+ * statistics are the call's own (reduce is never called).  The workspace sizes do not depend on it.
  * moments: caller-owned DEVICE buffer of 2*C_out + 1 doubles.  Forward: [sum a | sum a^2 | count] over the
- *   positions this rank normalises (EdgeConv: the B*N*k edge activations, MRConv: the B*N node activations);
- *   backward: [sum g | sum g*ahat | count] over the same positions.
+ *   positions this rank normalises (EdgeConv: the B*N*k edge activations, MRConv: the B*N node activations, the
+ *   sparse EdgeConv: the rank's E edge rows of z, E = 0 included);
+ *   backward: [sum g | sum g*ahat | count] over the same positions (the sparse EdgeConv then divides the first
+ *   2*C_out entries by the global count in place).
  * reduce(user): called on the calling host thread once per call, after the library has enqueued the LOCAL
  *   values into `moments` on `stream` and before it enqueues the work that reads them.  It must enqueue the
  *   element-wise sum of `moments` over all ranks (an all-reduce, in place) in the stream order of `stream` and
@@ -383,23 +385,30 @@ int dgcn_res_plus_backward_dh(const float* g_y, const float* h, int64_t N, int64
  * x (N, C_in) row-major fp32; the graph is dgcn_csr_build's rowptr (N+1) / src (E) of the edge_index (rows =
  * targets, edges in edge_index order); p: the MLP's parameters in dgcn_basic_conv (weight = the Linear's
  * (C_out, 2*C_in) weight, bn_* = the BatchNorm1d's); out (N, C_out) row-major fp32.
+ * sync: dgcn_bn_sync or NULL; with DGCN_NORM_BATCH_TRAIN the statistics are those of the edge rows of every rank.
+ * A rank with E = 0 still makes its reduce call.  N <= 0 is DGCN_ERR_BAD_ARG before any reduce call, so a synced
+ * rank without nodes leaves its peers waiting in their all-reduce: every rank must hold at least one node.
  * N <= 65535 * 32; ws: dgcn_sparse_edge_conv_workspace_bytes(N, C_in, C_out). */
 size_t dgcn_sparse_edge_conv_workspace_bytes(int64_t N, int64_t C_in, int64_t C_out);
 int dgcn_sparse_edge_conv_forward(const float* x, int64_t N, int64_t C_in, const int32_t* rowptr,
                                   const int32_t* src, int64_t E, const dgcn_basic_conv* p, int64_t C_out,
-                                  float* out, void* ws, size_t ws_bytes, dgcn_stream_t stream);
+                                  float* out, const dgcn_bn_sync* sync /* may be NULL */, void* ws, size_t ws_bytes,
+                                  dgcn_stream_t stream);
 /* Gradient of dgcn_sparse_edge_conv_forward w.r.t. x and the MLP's parameters (what torch autograd derives for the
  * reference, with the max's gradient going to the first edge in edge_index order that attains it, per node and
  * channel, as torch_scatter's scatter_max).  With DGCN_NORM_BATCH_TRAIN, p->bn_mean / p->bn_var must hold the
  * BATCH statistics the forward returned.  grad_x (N, C_in), grad_weight (C_out, 2*C_in), grad_bias (C_out),
  * grad_bn_weight / grad_bn_bias (C_out), grad_prelu (1) are OVERWRITTEN; any of them may be NULL.
+ * sync: dgcn_bn_sync or NULL, as in the forward; grad_x then comes from the sums and count of every rank, the
+ * parameter gradients stay this rank's.
  * ws: dgcn_sparse_edge_conv_backward_workspace_bytes(N, C_in, C_out). */
 size_t dgcn_sparse_edge_conv_backward_workspace_bytes(int64_t N, int64_t C_in, int64_t C_out);
 int dgcn_sparse_edge_conv_backward(const float* x, int64_t N, int64_t C_in, const int32_t* rowptr,
                                    const int32_t* src, int64_t E, const dgcn_basic_conv* p, int64_t C_out,
                                    const float* grad_out, float* grad_x, float* grad_weight, float* grad_bias,
-                                   float* grad_bn_weight, float* grad_bn_bias, float* grad_prelu, void* ws,
-                                   size_t ws_bytes, dgcn_stream_t stream);
+                                   float* grad_bn_weight, float* grad_bn_bias, float* grad_prelu,
+                                   const dgcn_bn_sync* sync /* may be NULL */, void* ws, size_t ws_bytes,
+                                   dgcn_stream_t stream);
 
 /* Halo packing for node-partitioned graphs (new functionality; the reference
  * has no multi-GPU sparse path, SURVEY.md 3.4): out[r,:] = x[rows[r],:].

@@ -327,11 +327,20 @@ class ConvParams:
         self.sync_group = sync_group if norm == NORM_BATCH_TRAIN else None
         self.moments = None
 
-    def bn_sync(self, dev):
-        """_BnSync for one forward or backward call, or None on the local-statistics path."""
-        if self.sync_group is None:
-            return None
-        return _BnSync(self.sync_group, self.weight.shape[0], dev)
+    def backward_stats(self):
+        """(mean, var) the backward normalises with: the forward's batch statistics in train mode, else the running
+        ones."""
+        return (self.batch_mean, self.batch_var) if self.norm == NORM_BATCH_TRAIN else (self.bn_mean, self.bn_var)
+
+    def grad_buffers(self, x_shape, dev, need_x=True):
+        """The gradients a backward writes, in the order of the C ABI's gradient arguments: x (of shape x_shape,
+        when need_x), weight, and bias, BatchNorm affine and PReLU weight where the layer has them."""
+        f = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)
+        c_out, bn = self.weight.shape[0], self.norm != NORM_NONE
+        return {"x": f(*x_shape) if need_x else None, "weight": f(*self.weight.shape),
+                "bias": f(c_out) if self.bias is not None else None,
+                "bn_weight": f(c_out) if bn else None, "bn_bias": f(c_out) if bn else None,
+                "prelu": f(1) if self.prelu_weight is not None else None}
 
     def tensors(self):
         return (self.weight, self.bias, self.prelu_weight, self.bn_weight, self.bn_bias, self.bn_mean, self.bn_var)
@@ -353,6 +362,17 @@ class ConvParams:
             self.batch_var = torch.empty(c_out, dtype=torch.float32, device=dev)
             s.batch_mean_out, s.batch_var_out = _ptr(self.batch_mean), _ptr(self.batch_var)
         return s
+
+
+def _basic_conv_call(fn, prm, nbytes, dev, *args):
+    """fn(*args, sync, ws, ws_bytes, stream), the call every BasicConv entry point ends with, in a workspace of nbytes.
+    With prm.sync_group the call gets a dgcn_bn_sync, and a failed reduce is raised with the all-reduce's exception as
+    its cause.  Returns the cross-rank moments of a synced call, else None."""
+    bs = None if prm.sync_group is None else _BnSync(prm.sync_group, prm.weight.shape[0], dev)
+    ws = _workspace(nbytes, dev)
+    rc = fn(*args, None if bs is None else ctypes.byref(bs.c), _ptr(ws), ws.numel(), _stream(dev))
+    (_check if bs is None else bs.check)(rc, fn.__name__)
+    return None if bs is None else bs.moments
 
 
 def knn_graph(x, k, dilation=1, cols=None, exclude_self=False, want_edge_index=True, want_nbr=False):
@@ -393,14 +413,10 @@ def graph_conv_forward(conv, x, prm, edge_index=None, nbr=None):
         l = lib()
         cs = prm.c_struct(dev)
         out = torch.empty((B, c_out, N, 1), dtype=torch.float32, device=dev)
-        ws = _workspace(l.dgcn_graph_conv_workspace_bytes(CONV[conv], B, C, c_out, N, k), dev)
-        bs = prm.bn_sync(dev)
-        rc = l.dgcn_graph_conv_forward(CONV[conv], _ptr(x3), B, C, N, sb, sc, _ptr(edge_index), _ptr(nbr), k,
-                                       ctypes.byref(cs), c_out, _ptr(out), None if bs is None else ctypes.byref(bs.c),
-                                       _ptr(ws), ws.numel(), _stream(dev))
-        (_check if bs is None else bs.check)(rc, "dgcn_graph_conv_forward")
-        if bs is not None:
-            prm.moments = bs.moments
+        prm.moments = _basic_conv_call(l.dgcn_graph_conv_forward, prm,
+                                       l.dgcn_graph_conv_workspace_bytes(CONV[conv], B, C, c_out, N, k), dev,
+                                       CONV[conv], _ptr(x3), B, C, N, sb, sc, _ptr(edge_index), _ptr(nbr), k,
+                                       ctypes.byref(cs), c_out, _ptr(out))
     return out
 
 
@@ -436,16 +452,12 @@ def dyn_conv_forward(conv, x, prm, k, dilation=1, cols=None, want_nbr=False, res
         if out is None:
             out = torch.empty((B, c_out, N, 1), dtype=torch.float32, device=dev)
         nbr = torch.empty((B, N, k), dtype=torch.int32, device=dev) if want_nbr else None
-        ws = _workspace(l.dgcn_dyn_conv_workspace_bytes(CONV[conv], B, C, c_out, N, K), dev)
-        bs = prm.bn_sync(dev)
-        if bs is not None and fus is not None:
+        if prm.sync_group is not None and fus is not None:
             raise RuntimeError("dyn_conv_forward: the block epilogue does not run with train-mode BatchNorm")
-        rc = l.dgcn_dyn_conv_forward(CONV[conv], _ptr(x3), B, C, N, sb, sc, ctypes.byref(dil), ctypes.byref(cs), c_out,
-                                     _ptr(out), _ptr(nbr), None if fus is None else ctypes.byref(fus),
-                                     None if bs is None else ctypes.byref(bs.c), _ptr(ws), ws.numel(), _stream(dev))
-        (_check if bs is None else bs.check)(rc, "dgcn_dyn_conv_forward")
-        if bs is not None:
-            prm.moments = bs.moments
+        prm.moments = _basic_conv_call(l.dgcn_dyn_conv_forward, prm,
+                                       l.dgcn_dyn_conv_workspace_bytes(CONV[conv], B, C, c_out, N, K), dev,
+                                       CONV[conv], _ptr(x3), B, C, N, sb, sc, ctypes.byref(dil), ctypes.byref(cs),
+                                       c_out, _ptr(out), _ptr(nbr), None if fus is None else ctypes.byref(fus))
     return out, nbr
 
 
@@ -464,24 +476,13 @@ def graph_conv_backward(conv, x, prm, grad_out, edge_index=None, nbr=None, need_
         k = nbr.shape[-1]
     with torch.cuda.device(dev):
         l = lib()
-        # train mode: the statistics of the batch the forward normalised with
-        stats = (prm.batch_mean, prm.batch_var) if prm.norm == NORM_BATCH_TRAIN else (prm.bn_mean, prm.bn_var)
-        cs = prm.c_struct(dev, stats)
-        f = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)
-        g = {"x": f(B, C, N) if need_x else None, "weight": f(c_out, 2 * C),
-             "bias": f(c_out) if prm.bias is not None else None,
-             "bn_weight": f(c_out) if prm.norm != NORM_NONE else None,
-             "bn_bias": f(c_out) if prm.norm != NORM_NONE else None,
-             "prelu": f(1) if prm.prelu_weight is not None else None}
-        ws = _workspace(l.dgcn_graph_conv_backward_workspace_bytes(CONV[conv], B, C, c_out, N, k), dev)
-        bs = prm.bn_sync(dev)
-        grads = (_ptr(g["x"]), _ptr(g["weight"]), _ptr(g["bias"]), _ptr(g["bn_weight"]), _ptr(g["bn_bias"]),
-                 _ptr(g["prelu"]))
+        cs = prm.c_struct(dev, prm.backward_stats())
+        g = prm.grad_buffers((B, C, N), dev, need_x)
         # synced: dx from the cross-rank sums; the parameter gradients stay local (SyncBatchNorm)
-        rc = l.dgcn_graph_conv_backward(CONV[conv], _ptr(x3), B, C, N, sb, sc, _ptr(edge_index), _ptr(nbr), k,
-                                        ctypes.byref(cs), c_out, _ptr(go), *grads,
-                                        None if bs is None else ctypes.byref(bs.c), _ptr(ws), ws.numel(), _stream(dev))
-        (_check if bs is None else bs.check)(rc, "dgcn_graph_conv_backward")
+        _basic_conv_call(l.dgcn_graph_conv_backward, prm,
+                         l.dgcn_graph_conv_backward_workspace_bytes(CONV[conv], B, C, c_out, N, k), dev,
+                         CONV[conv], _ptr(x3), B, C, N, sb, sc, _ptr(edge_index), _ptr(nbr), k, ctypes.byref(cs),
+                         c_out, _ptr(go), *map(_ptr, g.values()))
     return g
 
 
@@ -541,14 +542,10 @@ def sparse_edge_conv_forward(x, csr, E, prm):
         l = lib()
         cs = prm.c_struct(dev)
         out = torch.empty((N, c_out), dtype=torch.float32, device=dev)
-        ws = _workspace(l.dgcn_sparse_edge_conv_workspace_bytes(N, C, c_out), dev)
-        bs = prm.bn_sync(dev)
-        rc = l.dgcn_sparse_edge_conv_forward(_ptr(x), N, C, _ptr(rowptr), _ptr(src), int(E), ctypes.byref(cs), c_out,
-                                             _ptr(out), None if bs is None else ctypes.byref(bs.c), _ptr(ws),
-                                             ws.numel(), _stream(dev))
-        (_check if bs is None else bs.check)(rc, "dgcn_sparse_edge_conv_forward")
-        if bs is not None:
-            prm.moments = bs.moments
+        prm.moments = _basic_conv_call(l.dgcn_sparse_edge_conv_forward, prm,
+                                       l.dgcn_sparse_edge_conv_workspace_bytes(N, C, c_out), dev,
+                                       _ptr(x), N, C, _ptr(rowptr), _ptr(src), int(E), ctypes.byref(cs), c_out,
+                                       _ptr(out))
     return out
 
 
@@ -562,23 +559,13 @@ def sparse_edge_conv_backward(x, csr, E, prm, grad_out, need_x=True):
     go = _f32(grad_out)
     with torch.cuda.device(dev):
         l = lib()
-        stats = (prm.batch_mean, prm.batch_var) if prm.norm == NORM_BATCH_TRAIN else (prm.bn_mean, prm.bn_var)
-        cs = prm.c_struct(dev, stats)
-        f = lambda *shape: torch.empty(shape, dtype=torch.float32, device=dev)
-        g = {"x": f(N, C) if need_x else None, "weight": f(c_out, 2 * C),
-             "bias": f(c_out) if prm.bias is not None else None,
-             "bn_weight": f(c_out) if prm.norm != NORM_NONE else None,
-             "bn_bias": f(c_out) if prm.norm != NORM_NONE else None,
-             "prelu": f(1) if prm.prelu_weight is not None else None}
-        ws = _workspace(l.dgcn_sparse_edge_conv_backward_workspace_bytes(N, C, c_out), dev)
-        bs = prm.bn_sync(dev)
+        cs = prm.c_struct(dev, prm.backward_stats())
+        g = prm.grad_buffers((N, C), dev, need_x)
         # synced: dx from the cross-rank sums; the parameter gradients stay local (SyncBatchNorm)
-        rc = l.dgcn_sparse_edge_conv_backward(_ptr(x), N, C, _ptr(rowptr), _ptr(src), int(E), ctypes.byref(cs), c_out,
-                                              _ptr(go), _ptr(g["x"]), _ptr(g["weight"]), _ptr(g["bias"]),
-                                              _ptr(g["bn_weight"]), _ptr(g["bn_bias"]), _ptr(g["prelu"]),
-                                              None if bs is None else ctypes.byref(bs.c), _ptr(ws), ws.numel(),
-                                              _stream(dev))
-        (_check if bs is None else bs.check)(rc, "dgcn_sparse_edge_conv_backward")
+        _basic_conv_call(l.dgcn_sparse_edge_conv_backward, prm,
+                         l.dgcn_sparse_edge_conv_backward_workspace_bytes(N, C, c_out), dev,
+                         _ptr(x), N, C, _ptr(rowptr), _ptr(src), int(E), ctypes.byref(cs), c_out, _ptr(go),
+                         *map(_ptr, g.values()))
     return g
 
 

@@ -210,7 +210,7 @@ __device__ __forceinline__ BnMoments bn_load_partial(const float* partial, int64
 constexpr int TILE = 128;   // rows and cols of an output tile
 constexpr int TK = 16;      // k-chunk staged per step
 constexpr int NTHREADS = 256;
-constexpr int KCH = 512;     // points per CTA of the split-K weight-gradient GEMM (wgrad_kernel, dense_bwd.cu)
+constexpr int KCH = 512;     // points per CTA of the split-K weight-gradient GEMM (wgrad_kernel, basic_conv.cu)
 
 struct KMajor {          // a k-major operand: element (k, i) at ptr[k*ld + i]
   const float* ptr;      // rows k < K1

@@ -2,26 +2,16 @@
 // w.r.t. x and the BasicConv parameters - what torch autograd derives for
 // gcn_lib/dense/torch_vertex.py:16-35 + gcn_lib/dense/torch_nn.py:48-58.
 //
-// EdgeConv (factorised, see dense_fwd.cu): z_e = P[i'] + Q[j], a_e = act(z_e), y_e = s a_e + t,
+// EdgeConv (factorised, see basic_conv.cu): z_e = P[i'] + Q[j], a_e = act(z_e), y_e = s a_e + t,
 // out_i = max_e y_e.  The max routes grad_out to one edge per (i, channel); eval-mode BN keeps
 // it there, train-mode BN spreads it over every edge of the batch:
 //   da_e = s (g_e - dbeta/n - ahat_e dgamma/n),   dz_e = act'(z_e) da_e,
 //   dPQ[i'] += dz_e (P half), dPQ[j] += dz_e (Q half), then two node-level GEMMs.
 // MRConv: r_i = max_j x_j - x_i, z = W [x; r] + b: node-level BN/act backward, GEMMs, and a
 // scatter of dr through the per-channel argmax.
-#include "common.cuh"
+#include "basic_conv.cuh"
 
 namespace dgcn {
-
-float act_slope_of(const dgcn_basic_conv* p);
-__global__ void pack_edge_weights_kernel(const float* __restrict__ w, const float* __restrict__ bias, int ci, int co,
-                                         float* __restrict__ wk, float* __restrict__ bk);
-__global__ void pack_mr_weights_kernel(const float* __restrict__ w, int ci2, int co, float* __restrict__ wk);
-__global__ void to_node_major_kernel(const float* __restrict__ x, int64_t sb, int64_t sc, int C, int N,
-                                     float* __restrict__ xt);
-__global__ void node_pq_kernel(const float* __restrict__ x, int64_t sb, int64_t sc, int C, int N, int vec,
-                               const float* __restrict__ wk, const float* __restrict__ bk, int M,
-                               float* __restrict__ pq);
 
 struct EdgeBwdArgs {
   const float* pq;            // (B,N,2co) node-major, recomputed
@@ -130,43 +120,6 @@ __global__ void __launch_bounds__(256) edge_bwd_kernel(const EdgeBwdArgs g) {
   }
 }
 
-// fixed-order reduction of [np][nq][C] partials -> sums[nq][C] (double)
-__global__ void reduce_partials_kernel(const float* __restrict__ partial, int64_t np, int nq, int C,
-                                       double* __restrict__ sums) {
-  __shared__ double r[256];
-  const int c = blockIdx.x, q = blockIdx.y;
-  double a = 0.0;
-  for (int64_t i = threadIdx.x; i < np; i += blockDim.x) a += static_cast<double>(partial[(i * nq + q) * C + c]);
-  r[threadIdx.x] = a;
-  __syncthreads();
-  for (int o = blockDim.x >> 1; o > 0; o >>= 1) {
-    if (threadIdx.x < o) r[threadIdx.x] += r[threadIdx.x + o];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) sums[q * C + c] = r[0];
-}
-
-__global__ void store_count_kernel(double* __restrict__ dst, double count) { *dst = count; }
-
-// Synced backward sums (dgcn_bn_sync): sync->moments = [the fixed-order fp64 sums of rows q = 0, 1 of the
-// [np][nq][C] partials | count], then the caller enqueues their cross-rank sum on `stream`.  (The forward's
-// statistics partials are (count, mean, M2) rows: bn_merge_kernel, dense_fwd.cu.)
-int bn_sync_moments(const float* partial, int64_t np, int nq, int C, double count, const dgcn_bn_sync* sync,
-                    cudaStream_t stream) {
-  reduce_partials_kernel<<<dim3(C, 2), 256, 0, stream>>>(partial, np, nq, C, sync->moments);
-  DGCN_LAUNCH_CHECK();
-  store_count_kernel<<<1, 1, 0, stream>>>(sync->moments + 2 * static_cast<int64_t>(C), count);
-  DGCN_LAUNCH_CHECK();
-  return sync->reduce(sync->user) == 0 ? DGCN_OK : DGCN_ERR_REDUCE;
-}
-
-// Synced backward: the pass-1 operand [sum g | sum g*ahat] / count from the cross-rank moments, so pass 1 runs with
-// inv_count = 1 and the global count never visits the host.
-__global__ void moments_over_count_kernel(const double* __restrict__ moments, int C, double* __restrict__ sums) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < 2 * C) sums[i] = moments[i] / moments[2 * C];
-}
-
 // Train mode, after pass 0 wrote its partials: sums[0..2C) = (sum g, sum g*ahat) of this rank, with *inv_count
 // left as is, or with sync the global sums already divided by the global count and *inv_count = 1.
 static int bn_bwd_pass0_sums(const float* partial, int64_t np, int C, double count, const dgcn_bn_sync* sync,
@@ -182,114 +135,6 @@ static int bn_bwd_pass0_sums(const float* partial, int64_t np, int C, double cou
   DGCN_LAUNCH_CHECK();
   *inv_count = 1.0;
   return DGCN_OK;
-}
-
-// gradients of the BN affine parameters and of the PReLU slope from the reduced sums
-__global__ void finish_param_grads_kernel(const double* __restrict__ sums, int C, int have_slope,
-                                          float* __restrict__ grad_bn_w, float* __restrict__ grad_bn_b,
-                                          float* __restrict__ grad_prelu) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c < C) {
-    if (grad_bn_b) grad_bn_b[c] = static_cast<float>(sums[c]);
-    if (grad_bn_w) grad_bn_w[c] = static_cast<float>(sums[C + c]);
-  }
-  if (grad_prelu && have_slope && blockIdx.x == 0 && threadIdx.x == 0) {
-    double t = 0.0;
-    for (int i = 0; i < C; ++i) t += sums[2 * C + i];
-    grad_prelu[0] = static_cast<float>(t);
-  }
-}
-
-// C[r][c] = sum_k A[k][r] B[k][c]: generic node-level GEMM on the tile engine, plain store.
-__global__ void __launch_bounds__(NTHREADS, 2)
-    tile_gemm_kernel(KMajor A, int64_t a_batch, KMajor Bm, int64_t b_batch, float* __restrict__ out, int64_t ldo,
-                     int64_t o_batch, int rows, int cols) {
-  __shared__ TileSmem ts;
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const int b = blockIdx.z, r0 = blockIdx.y * TILE, c0 = blockIdx.x * TILE;
-  A.ptr += b * a_batch;
-  Bm.ptr += b * b_batch;
-  float acc[8][8];
-  tile_product(ts, A, r0, Bm, c0, acc);
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int rr = r0 + tile_row(ty, i);
-    if (rr >= rows) continue;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int cc = c0 + tile_col(tx, j);
-      if (cc < cols) out[b * o_batch + rr * ldo + cc] = acc[i][j];
-    }
-  }
-}
-
-// Split-K "both operands k-contiguous" GEMM for weight gradients:
-//   out[r][c] += sum_{b, n in chunk} A[b][r][n] * Bm[b][c][n]      (atomicAdd, out zero-initialised)
-// one CTA = one 128x128 output tile x one chunk of KCH points of one cloud (common.cuh).
-__global__ void __launch_bounds__(NTHREADS, 2)
-    wgrad_kernel(const float* __restrict__ A, int64_t a_batch, int64_t lda, int rows, const float* __restrict__ Bm,
-                 int64_t b_batch, int64_t ldb, int cols, int N, float* __restrict__ out, int64_t ldo) {
-  __shared__ TileSmem ts;
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const int b = blockIdx.z, n0 = blockIdx.x * KCH;
-  const int r0 = (blockIdx.y / ((cols + TILE - 1) / TILE)) * TILE, c0 = (blockIdx.y % ((cols + TILE - 1) / TILE)) * TILE;
-  const float* Ab = A + b * a_batch;
-  const float* Bb = Bm + b * b_batch;
-  float acc[8][8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
-  const int nend = min(N, n0 + KCH);
-  for (int k0 = n0; k0 < nend; k0 += TK) {
-    // transpose-load: element (k, i) of the chunk comes from src[i*ld + k]
-    for (int f = tid; f < TK * TILE; f += NTHREADS) {
-      const int kk = f & (TK - 1), i = f >> 4;
-      const int n = k0 + kk;
-      ts.a[0][kk][i] = (r0 + i < rows && n < nend) ? __ldg(Ab + static_cast<int64_t>(r0 + i) * lda + n) : 0.f;
-      ts.b[0][kk][i] = (c0 + i < cols && n < nend) ? __ldg(Bb + static_cast<int64_t>(c0 + i) * ldb + n) : 0.f;
-    }
-    __syncthreads();
-    chunk_fma(ts.a[0], ts.b[0], tx, ty, acc);
-    __syncthreads();
-  }
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int rr = r0 + tile_row(ty, i);
-    if (rr >= rows) continue;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int cc = c0 + tile_col(tx, j);
-      if (cc < cols) atomicAdd(out + rr * ldo + cc, acc[i][j]);
-    }
-  }
-}
-
-// EdgeConv: dWcat (2co x ci) -> grad_weight (co x 2ci): W1 = dA, W2 = dW2f - dA; bias from dpq row sums
-__global__ void unpack_edge_wgrad_kernel(const float* __restrict__ dwcat, int ci, int co, float* __restrict__ gw) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= co * ci) return;
-  const int m = i / ci, c = i % ci;
-  const float da = dwcat[m * ci + c], dw2 = dwcat[(co + m) * ci + c];
-  gw[m * 2 * ci + c] = da;
-  gw[m * 2 * ci + ci + c] = dw2 - da;
-}
-// row sums over (b, n) of a (B, M, N) tensor, rows [0, rows): one block per row
-__global__ void row_sum_kernel(const float* __restrict__ t, int B, int M, int N, int rows, float* __restrict__ out) {
-  __shared__ double r[256];
-  const int m = blockIdx.x;
-  double a = 0.0;
-  for (int64_t i = threadIdx.x; i < static_cast<int64_t>(B) * N; i += blockDim.x) {
-    const int b = static_cast<int>(i / N), n = static_cast<int>(i % N);
-    a += static_cast<double>(t[(static_cast<int64_t>(b) * M + m) * N + n]);
-  }
-  r[threadIdx.x] = a;
-  __syncthreads();
-  for (int o = blockDim.x >> 1; o > 0; o >>= 1) {
-    if (threadIdx.x < o) r[threadIdx.x] += r[threadIdx.x + o];
-    __syncthreads();
-  }
-  if (threadIdx.x == 0 && m < rows) out[m] = static_cast<float>(r[0]);
 }
 
 // ---- MRConv pieces --------------------------------------------------------------------------------------
@@ -457,10 +302,10 @@ int dgcn_graph_conv_backward(int32_t conv, const float* x, int64_t B, int64_t ci
                              float* grad_bn_weight, float* grad_bn_bias, float* grad_prelu, const dgcn_bn_sync* sync,
                              void* wsp, size_t ws_bytes, dgcn_stream_t stream_) {
   if (conv != DGCN_CONV_EDGE && conv != DGCN_CONV_MR) return DGCN_ERR_UNSUPPORTED;
-  if (!x || !p || !p->weight || !grad_out || (!edge_index && !nbr) || B <= 0 || ci <= 0 || co <= 0 || N <= 0 || k <= 0)
+  if (!x || !grad_out || (!edge_index && !nbr) || B <= 0 || ci <= 0 || co <= 0 || N <= 0 || k <= 0)
     return DGCN_ERR_BAD_ARG;
-  if (p->norm != DGCN_NORM_NONE && (!p->bn_mean || !p->bn_var)) return DGCN_ERR_BAD_ARG;
-  if (sync && (!sync->moments || !sync->reduce)) return DGCN_ERR_BAD_ARG;
+  int rc = check_basic_conv(p, sync, true);
+  if (rc != DGCN_OK) return rc;
   if (B > 65535 || co > 65535) return DGCN_ERR_UNSUPPORTED;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   Workspace ws(wsp, ws_bytes);
@@ -497,8 +342,8 @@ int dgcn_graph_conv_backward(int32_t conv, const float* x, int64_t B, int64_t ci
     if (train) {
       edge_bwd_kernel<0><<<grid, 256, 0, stream>>>(g);
       DGCN_LAUNCH_CHECK();
-      int rc = bn_bwd_pass0_sums(partial, w.n_partial, ico, static_cast<double>(B) * N * k, sync, sums, &g1.inv_count,
-                                 stream);
+      rc = bn_bwd_pass0_sums(partial, w.n_partial, ico, static_cast<double>(B) * N * k, sync, sums, &g1.inv_count,
+                             stream);
       if (rc != DGCN_OK) return rc;
       // pass B wants (dbeta, dgamma) as float[2][co]: finish_param_grads_kernel does the conversion
       finish_param_grads_kernel<<<static_cast<unsigned>(ceil_div(co, 128)), 128, 0, stream>>>(sums, ico, 0, w.sf + co,
@@ -525,21 +370,7 @@ int dgcn_graph_conv_backward(int32_t conv, const float* x, int64_t B, int64_t ci
           A, 0, Bm, static_cast<int64_t>(M) * N, grad_x, N, ci * N, ici, iN);
       DGCN_LAUNCH_CHECK();
     }
-    if (grad_weight) {
-      DGCN_CUDA_TRY(cudaMemsetAsync(dwcat, 0, static_cast<size_t>(M) * ci * sizeof(float), stream));
-      const int tiles = static_cast<int>(ceil_div(M, TILE) * ceil_div(ci, TILE));
-      wgrad_kernel<<<dim3(ceil_div(N, KCH), tiles, B), NTHREADS, 0, stream>>>(dpq, static_cast<int64_t>(M) * N, N, M, x,
-                                                                            sb, sc, ici, iN, dwcat, ci);
-      DGCN_LAUNCH_CHECK();
-      unpack_edge_wgrad_kernel<<<static_cast<unsigned>(ceil_div(co * ci, 256)), 256, 0, stream>>>(dwcat, ici, ico,
-                                                                                                grad_weight);
-      DGCN_LAUNCH_CHECK();
-    }
-    if (grad_bias) {
-      row_sum_kernel<<<ico, 256, 0, stream>>>(dpq, iB, M, iN, ico, grad_bias);
-      DGCN_LAUNCH_CHECK();
-    }
-    return DGCN_OK;
+    return edge_param_grads(dpq, x, sb, sc, B, ci, co, N, dwcat, grad_weight, grad_bias, stream);
   }
 
   // ---- MRConv ---------------------------------------------------------------------------------------------
@@ -579,7 +410,7 @@ int dgcn_graph_conv_backward(int32_t conv, const float* x, int64_t B, int64_t ci
   if (train) {
     mr_bn_bwd_kernel<0><<<bgrid, 256, 0, stream>>>(mb);
     DGCN_LAUNCH_CHECK();
-    int rc = bn_bwd_pass0_sums(partial, w.n_partial, ico, static_cast<double>(B) * N, sync, sums, &mb.inv_count, stream);
+    rc = bn_bwd_pass0_sums(partial, w.n_partial, ico, static_cast<double>(B) * N, sync, sums, &mb.inv_count, stream);
     if (rc != DGCN_OK) return rc;
   }
   mr_bn_bwd_kernel<1><<<bgrid, 256, 0, stream>>>(mb);   // z now holds dz

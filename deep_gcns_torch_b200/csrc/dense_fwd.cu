@@ -4,6 +4,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <stdio.h>
+#include "basic_conv.cuh"
 #include "knn_tc4.cuh"
 
 namespace dgcn {
@@ -437,71 +438,6 @@ int fill_knn_args(KnnArgs& a, const float* x, int64_t B, int64_t C, int64_t N, i
   return DGCN_OK;
 }
 
-// ---- node-level kernels ---------------------------------------------------------------
-// EdgeConv weight split (SURVEY.md 7): W.[x_i ; x_j - x_i] = (W1 - W2) x_i + W2 x_j.
-// wk[c][m] (k-major, m < 2*co): m < co -> W1[m][c] - W2[m][c]; else W2[m-co][c].  bk = (bias | 0).
-__global__ void pack_edge_weights_kernel(const float* __restrict__ w, const float* __restrict__ bias,
-                                         int ci, int co, float* __restrict__ wk, float* __restrict__ bk) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < ci * 2 * co) {
-    int c = i / (2 * co), m = i % (2 * co);
-    float v;
-    if (m < co) v = w[m * 2 * ci + c] - w[m * 2 * ci + ci + c];
-    else v = w[(m - co) * 2 * ci + ci + c];
-    wk[i] = v;
-  }
-  if (i < 2 * co) bk[i] = (i < co && bias) ? bias[i] : 0.f;
-}
-// MRConv weight transpose: wk[kk][m] = W[m][kk], kk < 2*ci
-__global__ void pack_mr_weights_kernel(const float* __restrict__ w, int ci2, int co, float* __restrict__ wk) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < ci2 * co) {
-    int kk = i / co, m = i % co;
-    wk[i] = w[m * ci2 + kk];
-  }
-}
-
-// (B,C,N) strided -> (B,N,C) contiguous
-__global__ void to_node_major_kernel(const float* __restrict__ x, int64_t sb, int64_t sc, int C, int N,
-                                     float* __restrict__ xt) {
-  __shared__ float t[32][33];
-  const int b = blockIdx.z, n0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
-  for (int r = threadIdx.y; r < 32; r += blockDim.y) {
-    int c = c0 + r, n = n0 + threadIdx.x;
-    t[r][threadIdx.x] = (c < C && n < N) ? __ldg(x + b * sb + c * sc + n) : 0.f;
-  }
-  __syncthreads();
-  for (int r = threadIdx.y; r < 32; r += blockDim.y) {
-    int n = n0 + r, c = c0 + threadIdx.x;
-    if (n < N && c < C) xt[(static_cast<int64_t>(b) * N + n) * C + c] = t[threadIdx.x][r];
-  }
-}
-
-// PQ[b][n][m] = sum_c X[b][c][n] * wk[c][m] + bk[m]      (rows = points, cols = m)
-__global__ void __launch_bounds__(NTHREADS, 2)
-    node_pq_kernel(const float* __restrict__ x, int64_t sb, int64_t sc, int C, int N, int vec,
-                   const float* __restrict__ wk, const float* __restrict__ bk, int M,
-                   float* __restrict__ pq) {
-  __shared__ TileSmem ts;
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const int b = blockIdx.z, n0 = blockIdx.y * TILE, m0 = blockIdx.x * TILE;
-  KMajor A = kmajor1(x + b * sb, sc, C, N, vec != 0);
-  KMajor Bm = kmajor1(wk, M, C, M, (M % 4) == 0);
-  float acc[8][8];
-  tile_product(ts, A, n0, Bm, m0, acc);
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int n = n0 + tile_row(ty, i);
-    if (n >= N) continue;
-    float* row = pq + (static_cast<int64_t>(b) * N + n) * M;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int m = m0 + tile_col(tx, j);
-      if (m < M) row[m] = acc[i][j] + __ldg(bk + m);
-    }
-  }
-}
-
 // MRConv node update: out[b][m][n] = norm(act(sum_kk wk[kk][m] * [x ; r][kk][n] + bias[m]))
 // rows = m, cols = points.  Train mode stores act() and per-CTA partial statistics.
 struct MrNodeArgs {
@@ -554,103 +490,6 @@ __global__ void __launch_bounds__(NTHREADS, 2) mr_node_kernel(const MrNodeArgs g
       if (tx == 0 && m < g.co) bn_store_partial(g.partial, static_cast<int64_t>(b) * gridDim.x + blockIdx.x, g.co, m, mo);
     }
   }
-}
-
-// Channel c's batch mean and biased variance -> (scale, shift), and both for the host's running-stat update
-// (torch BatchNorm2d training semantics: normalise with biased variance).
-__device__ __forceinline__ void bn_finalize_channel(double mean, double var, int C, int c,
-                                                    const float* __restrict__ bn_w, const float* __restrict__ bn_b,
-                                                    float eps, float* __restrict__ st, float* __restrict__ mean_out,
-                                                    float* __restrict__ var_out) {
-  if (var < 0.0) var = 0.0;
-  float inv = 1.0f / sqrtf(static_cast<float>(var) + eps);
-  float s = (bn_w ? bn_w[c] : 1.f) * inv;
-  st[c] = s;
-  st[C + c] = (bn_b ? bn_b[c] : 0.f) - static_cast<float>(mean) * s;
-  if (mean_out) mean_out[c] = static_cast<float>(mean);
-  if (var_out) var_out[c] = static_cast<float>(var);
-}
-
-// fp64 Chan merge of two disjoint sets' (count, mean, M2); either may be empty
-__device__ __forceinline__ void bn_merge64(double& n, double& mean, double& m2, double nb, double meanb, double m2b) {
-  const double t = n + nb;
-  const double f = t > 0.0 ? nb / t : 0.0;
-  const double delta = meanb - mean;
-  m2 += m2b + delta * (delta * (n * f));
-  mean += delta * f;
-  n = t;
-}
-
-// Batch statistics from the [np][3][C] partial rows (common.cuh), merged in fp64 in a fixed order, one CTA per
-// channel.  Local statistics: (scale, shift), batch mean and variance.  Synced (moments != null): this rank's
-// [sum a | sum a^2 | count] of the dgcn_bn_sync ABI, formed in fp64 from the merged (count, mean, M2).
-__global__ void bn_merge_kernel(const float* __restrict__ partial, int64_t np, int C, double count,
-                                const float* __restrict__ bn_w, const float* __restrict__ bn_b, float eps,
-                                float* __restrict__ st, float* __restrict__ mean_out, float* __restrict__ var_out,
-                                double* __restrict__ moments) {
-  __shared__ double rn[256], rm[256], r2[256];
-  const int c = blockIdx.x;
-  double n = 0.0, mean = 0.0, m2 = 0.0;
-  for (int64_t i = threadIdx.x; i < np; i += blockDim.x) {
-    const BnMoments p = bn_load_partial(partial, i, C, c);
-    bn_merge64(n, mean, m2, p.n, p.mean, p.m2);
-  }
-  rn[threadIdx.x] = n;
-  rm[threadIdx.x] = mean;
-  r2[threadIdx.x] = m2;
-  __syncthreads();
-  for (int o = blockDim.x >> 1; o > 0; o >>= 1) {
-    if (threadIdx.x < o) {
-      n = rn[threadIdx.x];
-      mean = rm[threadIdx.x];
-      m2 = r2[threadIdx.x];
-      bn_merge64(n, mean, m2, rn[threadIdx.x + o], rm[threadIdx.x + o], r2[threadIdx.x + o]);
-      rn[threadIdx.x] = n;
-      rm[threadIdx.x] = mean;
-      r2[threadIdx.x] = m2;
-    }
-    __syncthreads();
-  }
-  if (threadIdx.x != 0) return;
-  n = rn[0];
-  mean = rm[0];
-  m2 = r2[0];
-  if (moments) {
-    const double s1 = n * mean;
-    moments[c] = s1;
-    moments[C + c] = m2 + s1 * mean;   // bn_finalize_moments_kernel subtracts the same product: M2 comes back exact
-    if (c == 0) moments[2 * C] = count;
-    return;
-  }
-  bn_finalize_channel(mean, n > 0.0 ? m2 / n : 0.0, C, c, bn_w, bn_b, eps, st, mean_out, var_out);
-}
-// Synced statistics (dgcn_bn_sync): the same finalisation from the cross-rank moments [sum a | sum a^2 | count],
-// the count read on the device.  After the all-reduce the fp64 cancellation costs ~ (mean / std)^2 * 2^-53.
-__global__ void bn_finalize_moments_kernel(const double* __restrict__ moments, int C, const float* __restrict__ bn_w,
-                                           const float* __restrict__ bn_b, float eps, float* __restrict__ st,
-                                           float* __restrict__ mean_out, float* __restrict__ var_out) {
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-  const double count = moments[2 * C], s1 = moments[c];
-  const double mean = s1 / count;
-  bn_finalize_channel(mean, (moments[C + c] - s1 * mean) / count, C, c, bn_w, bn_b, eps, st, mean_out, var_out);
-}
-
-// Train mode: (scale, shift) into st from the partial rows of `count` positions; with sync, from the
-// statistics of every rank.  Shared with the sparse EdgeConv (sparse_edge.cu).
-int bn_finalize(const float* partial, int64_t np, int64_t co, double count, const dgcn_basic_conv* p,
-                const dgcn_bn_sync* sync, float* st, cudaStream_t stream) {
-  const int C = static_cast<int>(co);
-  bn_merge_kernel<<<static_cast<unsigned>(co), 256, 0, stream>>>(partial, np, C, count, p->bn_weight, p->bn_bias,
-                                                                 p->bn_eps, st, p->batch_mean_out, p->batch_var_out,
-                                                                 sync ? sync->moments : nullptr);
-  DGCN_LAUNCH_CHECK();
-  if (!sync) return DGCN_OK;
-  if (sync->reduce(sync->user) != 0) return DGCN_ERR_REDUCE;
-  bn_finalize_moments_kernel<<<static_cast<unsigned>(ceil_div(co, 128)), 128, 0, stream>>>(
-      sync->moments, C, p->bn_weight, p->bn_bias, p->bn_eps, st, p->batch_mean_out, p->batch_var_out);
-  DGCN_LAUNCH_CHECK();
-  return DGCN_OK;
 }
 
 // out = s >= 0 ? s*out + t : s*out_min + t   (out_min may be null: plain affine)
@@ -785,24 +624,13 @@ static ConvRegions carve_conv(int conv, int64_t B, int64_t ci, int64_t co, int64
 }
 
 static int check_conv_args(int conv, const float* x, int64_t B, int64_t ci, int64_t N, const dgcn_basic_conv* p,
-                           int64_t co, const float* out) {
+                           int64_t co, const float* out, const dgcn_bn_sync* sync) {
   if (conv != DGCN_CONV_EDGE && conv != DGCN_CONV_MR) return DGCN_ERR_UNSUPPORTED;
-  if (!x || !p || !p->weight || !out || B <= 0 || ci <= 0 || co <= 0 || N <= 0) return DGCN_ERR_BAD_ARG;
-  if (p->act < DGCN_ACT_NONE || p->act > DGCN_ACT_PRELU) return DGCN_ERR_UNSUPPORTED;
-  if (p->act == DGCN_ACT_PRELU && !p->prelu_weight) return DGCN_ERR_BAD_ARG;
-  if (p->norm < DGCN_NORM_NONE || p->norm > DGCN_NORM_BATCH_TRAIN) return DGCN_ERR_UNSUPPORTED;
-  if (p->norm == DGCN_NORM_BATCH_EVAL && (!p->bn_mean || !p->bn_var)) return DGCN_ERR_BAD_ARG;
+  if (!x || !out || B <= 0 || ci <= 0 || co <= 0 || N <= 0) return DGCN_ERR_BAD_ARG;
+  const int rc = check_basic_conv(p, sync, false);
+  if (rc != DGCN_OK) return rc;
   if (B > 65535) return DGCN_ERR_UNSUPPORTED;
   return DGCN_OK;
-}
-
-float act_slope_of(const dgcn_basic_conv* p) {
-  switch (p->act) {
-    case DGCN_ACT_RELU: return 0.f;
-    case DGCN_ACT_LEAKYRELU: return p->slope;
-    case DGCN_ACT_PRELU: return 0.f;   // read from prelu_weight on device
-    default: return 1.f;
-  }
 }
 
 // Shared body of graph_conv_forward (graph given) and dyn_conv_forward (graph fused).
@@ -951,10 +779,9 @@ int dgcn_graph_conv_forward(int32_t conv, const float* x, int64_t B, int64_t C_i
                             int64_t stride_c, const int64_t* edge_index, const int32_t* nbr, int64_t k,
                             const dgcn_basic_conv* p, int64_t C_out, float* out, const dgcn_bn_sync* sync, void* wsp,
                             size_t ws_bytes, dgcn_stream_t stream) {
-  int rc = check_conv_args(conv, x, B, C_in, N, p, C_out, out);
+  int rc = check_conv_args(conv, x, B, C_in, N, p, C_out, out, sync);
   if (rc != DGCN_OK) return rc;
   if ((!edge_index && !nbr) || k <= 0) return DGCN_ERR_BAD_ARG;
-  if (sync && (!sync->moments || !sync->reduce)) return DGCN_ERR_BAD_ARG;
   Workspace ws(wsp, ws_bytes);
   return conv_forward(conv, x, B, C_in, N, stride_b, stride_c, edge_index, nbr, k, nullptr, p, C_out, out, nullptr,
                       ws, static_cast<cudaStream_t>(stream), nullptr, sync);
@@ -971,10 +798,9 @@ int dgcn_dyn_conv_forward(int32_t conv, const float* x, int64_t B, int64_t C_in,
                           int64_t stride_c, const dgcn_dilation* dil, const dgcn_basic_conv* p, int64_t C_out,
                           float* out, int32_t* nbr_out, const dgcn_block_fusion* fus, const dgcn_bn_sync* sync,
                           void* wsp, size_t ws_bytes, dgcn_stream_t stream) {
-  int rc = check_conv_args(conv, x, B, C_in, N, p, C_out, out);
+  int rc = check_conv_args(conv, x, B, C_in, N, p, C_out, out, sync);
   if (rc != DGCN_OK) return rc;
   if (!dil) return DGCN_ERR_BAD_ARG;
-  if (sync && (!sync->moments || !sync->reduce)) return DGCN_ERR_BAD_ARG;
   Workspace ws(wsp, ws_bytes);
   return conv_forward(conv, x, B, C_in, N, stride_b, stride_c, nullptr, nullptr, 0, dil, p, C_out, out, nbr_out, ws,
                       static_cast<cudaStream_t>(stream), fus, sync);

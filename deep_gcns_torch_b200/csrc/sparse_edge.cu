@@ -19,38 +19,11 @@
 // grad_x are node-level products of dPQ.
 //
 // Synced statistics (dgcn_bn_sync, nn.SyncBatchNorm): the forward all-reduces this rank's moments of z between the
-// edge pass and the (s, t) finalisation (dense_fwd.cu's bn_finalize); the backward all-reduces pass 0's sums, and
+// edge pass and the (s, t) finalisation (bn_finalize); the backward all-reduces pass 0's sums, and
 // pass 1 runs with the global sums over the global count.  The edge kernels are the same on both paths.
-#include "common.cuh"
+#include "basic_conv.cuh"
 
 namespace dgcn {
-
-float act_slope_of(const dgcn_basic_conv* p);
-__global__ void pack_edge_weights_kernel(const float* __restrict__ w, const float* __restrict__ bias, int ci, int co,
-                                         float* __restrict__ wk, float* __restrict__ bk);
-__global__ void pack_mr_weights_kernel(const float* __restrict__ w, int ci2, int co, float* __restrict__ wk);
-__global__ void to_node_major_kernel(const float* __restrict__ x, int64_t sb, int64_t sc, int C, int N,
-                                     float* __restrict__ xt);
-__global__ void node_pq_kernel(const float* __restrict__ x, int64_t sb, int64_t sc, int C, int N, int vec,
-                               const float* __restrict__ wk, const float* __restrict__ bk, int M,
-                               float* __restrict__ pq);
-__global__ void reduce_partials_kernel(const float* __restrict__ partial, int64_t np, int nq, int C,
-                                       double* __restrict__ sums);
-int bn_finalize(const float* partial, int64_t np, int64_t co, double count, const dgcn_basic_conv* p,
-                const dgcn_bn_sync* sync, float* st, cudaStream_t stream);
-int bn_sync_moments(const float* partial, int64_t np, int nq, int C, double count, const dgcn_bn_sync* sync,
-                    cudaStream_t stream);
-__global__ void moments_over_count_kernel(const double* __restrict__ moments, int C, double* __restrict__ sums);
-__global__ void finish_param_grads_kernel(const double* __restrict__ sums, int C, int have_slope,
-                                          float* __restrict__ grad_bn_w, float* __restrict__ grad_bn_b,
-                                          float* __restrict__ grad_prelu);
-__global__ void tile_gemm_kernel(KMajor A, int64_t a_batch, KMajor Bm, int64_t b_batch, float* __restrict__ out,
-                                 int64_t ldo, int64_t o_batch, int rows, int cols);
-__global__ void wgrad_kernel(const float* __restrict__ A, int64_t a_batch, int64_t lda, int rows,
-                             const float* __restrict__ Bm, int64_t b_batch, int64_t ldb, int cols, int N,
-                             float* __restrict__ out, int64_t ldo);
-__global__ void unpack_edge_wgrad_kernel(const float* __restrict__ dwcat, int ci, int co, float* __restrict__ gw);
-__global__ void row_sum_kernel(const float* __restrict__ t, int B, int M, int N, int rows, float* __restrict__ out);
 
 constexpr int SPE_WARPS = 8;            // warps per CTA of the edge passes
 constexpr int SPE_ROWS_PER_WARP = 4;    // CSR rows per warp
@@ -295,12 +268,11 @@ static SpEdgeRegions carve_sp_edge(bool backward, int64_t N, int64_t ci, int64_t
 }
 
 static int check_sp_edge_args(const float* x, int64_t N, int64_t ci, const int32_t* rowptr, const int32_t* src,
-                              int64_t E, const dgcn_basic_conv* p, int64_t co, const dgcn_bn_sync* sync) {
-  if (!x || !rowptr || !src || !p || !p->weight || N <= 0 || ci <= 0 || co <= 0 || E < 0) return DGCN_ERR_BAD_ARG;
-  if (sync && (!sync->moments || !sync->reduce)) return DGCN_ERR_BAD_ARG;
-  if (p->act < DGCN_ACT_NONE || p->act > DGCN_ACT_PRELU) return DGCN_ERR_UNSUPPORTED;
-  if (p->act == DGCN_ACT_PRELU && !p->prelu_weight) return DGCN_ERR_BAD_ARG;
-  if (p->norm < DGCN_NORM_NONE || p->norm > DGCN_NORM_BATCH_TRAIN) return DGCN_ERR_UNSUPPORTED;
+                              int64_t E, const dgcn_basic_conv* p, int64_t co, const dgcn_bn_sync* sync,
+                              bool backward) {
+  if (!x || !rowptr || !src || N <= 0 || ci <= 0 || co <= 0 || E < 0) return DGCN_ERR_BAD_ARG;
+  const int rc = check_basic_conv(p, sync, backward);
+  if (rc != DGCN_OK) return rc;
   if (N > SPE_MAX_N || E > INT32_MAX || co > 65535 || ci > 65535) return DGCN_ERR_UNSUPPORTED;
   return DGCN_OK;
 }
@@ -351,10 +323,9 @@ size_t dgcn_sparse_edge_conv_workspace_bytes(int64_t N, int64_t C_in, int64_t C_
 int dgcn_sparse_edge_conv_forward(const float* x, int64_t N, int64_t C_in, const int32_t* rowptr, const int32_t* src,
                                   int64_t E, const dgcn_basic_conv* p, int64_t C_out, float* out,
                                   const dgcn_bn_sync* sync, void* wsp, size_t ws_bytes, dgcn_stream_t stream_) {
-  int rc = check_sp_edge_args(x, N, C_in, rowptr, src, E, p, C_out, sync);
+  int rc = check_sp_edge_args(x, N, C_in, rowptr, src, E, p, C_out, sync, false);
   if (rc != DGCN_OK) return rc;
   if (!out) return DGCN_ERR_BAD_ARG;
-  if (p->norm == DGCN_NORM_BATCH_EVAL && (!p->bn_mean || !p->bn_var)) return DGCN_ERR_BAD_ARG;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const bool train = p->norm == DGCN_NORM_BATCH_TRAIN;
   Workspace ws(wsp, ws_bytes);
@@ -394,10 +365,9 @@ int dgcn_sparse_edge_conv_backward(const float* x, int64_t N, int64_t C_in, cons
                                    const float* grad_out, float* grad_x, float* grad_weight, float* grad_bias,
                                    float* grad_bn_weight, float* grad_bn_bias, float* grad_prelu,
                                    const dgcn_bn_sync* sync, void* wsp, size_t ws_bytes, dgcn_stream_t stream_) {
-  int rc = check_sp_edge_args(x, N, C_in, rowptr, src, E, p, C_out, sync);
+  int rc = check_sp_edge_args(x, N, C_in, rowptr, src, E, p, C_out, sync, true);
   if (rc != DGCN_OK) return rc;
   if (!grad_out) return DGCN_ERR_BAD_ARG;
-  if (p->norm != DGCN_NORM_NONE && (!p->bn_mean || !p->bn_var)) return DGCN_ERR_BAD_ARG;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const bool train = p->norm == DGCN_NORM_BATCH_TRAIN;
   Workspace ws(wsp, ws_bytes);
@@ -463,21 +433,8 @@ int dgcn_sparse_edge_conv_backward(const float* x, int64_t N, int64_t C_in, cons
         A, 0, Bm, 0, grad_x, C_in, 0, iN, ici);
     DGCN_LAUNCH_CHECK();
   }
-  if (grad_weight) {   // dWcat[m][c] = sum_n dPQ[n][m] x[n][c]; W1 = dA, W2 = dB - dA
-    DGCN_CUDA_TRY(cudaMemsetAsync(w.dwcat, 0, static_cast<size_t>(M) * C_in * sizeof(float), stream));
-    const int tiles = static_cast<int>(ceil_div(M, TILE) * ceil_div(C_in, TILE));
-    wgrad_kernel<<<dim3(ceil_div(N, KCH), tiles, 1), NTHREADS, 0, stream>>>(w.dpqt, 0, N, M, w.xt, 0, N,
-                                                                                     ici, iN, w.dwcat, C_in);
-    DGCN_LAUNCH_CHECK();
-    unpack_edge_wgrad_kernel<<<static_cast<unsigned>(ceil_div(C_out * C_in, 256)), 256, 0, stream>>>(w.dwcat, ici,
-                                                                                                   ico, grad_weight);
-    DGCN_LAUNCH_CHECK();
-  }
-  if (grad_bias) {   // db = sum_n dP_n
-    row_sum_kernel<<<ico, 256, 0, stream>>>(w.dpqt, 1, M, iN, ico, grad_bias);
-    DGCN_LAUNCH_CHECK();
-  }
-  return DGCN_OK;
+  // xt (ci, N) is x as one channel-major cloud
+  return edge_param_grads(w.dpqt, w.xt, 0, N, 1, C_in, C_out, N, w.dwcat, grad_weight, grad_bias, stream);
 }
 
 }  // extern "C"

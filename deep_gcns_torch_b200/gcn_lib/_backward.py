@@ -1,24 +1,6 @@
-"""Backward glue of the autograd nodes of the drop-in modules: unpack what forward saved,
-call the native gradient kernels (dgcn_graph_conv_backward / dgcn_genconv_aggregate_backward),
-hand the gradients back in the order of the forward's inputs."""
+"""Backward glue of GENConv's aggregate autograd node: unpack what forward saved, call the native gradient
+kernels (dgcn_genconv_aggregate_backward), hand the gradients back in the order of the forward's inputs."""
 from .. import _native
-
-
-def graph_conv_backward(ctx, grad_out):
-    """Inputs of _GraphConvFn.forward: (owner, x, edge_index, fused, weight, bias, prelu, bn_w, bn_b)."""
-    (x,) = ctx.saved_tensors
-    owner, prm = ctx.owner, ctx.prm
-    need = ctx.needs_input_grad
-    g = _native.graph_conv_backward(owner._conv, x, prm, grad_out, edge_index=ctx.edge_index,
-                                    nbr=None if ctx.edge_index is not None else ctx.nbr, need_x=need[1])
-    conv = owner.nn[0]
-    gx = g["x"].view(x.shape[0], x.shape[1], x.shape[2], 1) if need[1] else None
-    gw = g["weight"].view_as(conv.weight) if need[4] else None
-    gb = g["bias"] if (need[5] and g["bias"] is not None) else None
-    gp = g["prelu"] if (need[6] and g["prelu"] is not None) else None
-    gbw = g["bn_weight"] if (need[7] and g["bn_weight"] is not None) else None
-    gbb = g["bn_bias"] if (need[8] and g["bn_bias"] is not None) else None
-    return None, gx, None, None, gw, gb, gp, gbw, gbb
 
 
 def genconv_aggregate_backward(ctx, grad_out):

@@ -9,6 +9,7 @@ import torch
 from torch import nn
 
 from ... import _native
+from .._basic_conv import BasicConvLowering, update_running_stats
 from .torch_nn import BasicConv
 from .torch_edge import DenseDilatedKnnGraph, DilatedKnnGraph
 
@@ -22,27 +23,36 @@ class _GraphConvFn(torch.autograd.Function):
     every rank."""
 
     @staticmethod
-    def forward(ctx, owner, x, edge_index, fused, *params):
-        prm = owner._conv_params()
+    def forward(ctx, owner, parts, x, edge_index, fused, *params):
+        prm = owner._conv_params(parts)
         if fused is not None:                       # dynamic graph, built in the same launch sequence
             k, dilation, cols, need_graph = fused[:4]
             block = fused[4] if len(fused) > 4 else {}      # block epilogue (inference): residual / res_scale / out
             out, nbr = _native.dyn_conv_forward(owner._conv, x, prm, k, dilation, cols, want_nbr=need_graph, **block)
         else:
-            nbr = None
+            k, nbr = edge_index.shape[-1], None
             out = _native.graph_conv_forward(owner._conv, x, prm, edge_index=edge_index)
-        owner._after_forward(prm, x, out, edge_index.shape[-1] if fused is None else fused[0])
+        # EdgeConv normalises the B*N*k edge activations, MRConv the B*N node activations
+        update_running_stats(parts[3], prm, x.shape[0] * x.shape[2] * (k if owner._conv == "edge" else 1))
         ctx.owner, ctx.prm, ctx.nbr, ctx.edge_index = owner, prm, nbr, edge_index
         ctx.save_for_backward(x)
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
-        from .. import _backward
-        return _backward.graph_conv_backward(ctx, grad_out)
+        (x,) = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        g = _native.graph_conv_backward(ctx.owner._conv, x, ctx.prm, grad_out, edge_index=ctx.edge_index, nbr=ctx.nbr,
+                                        need_x=need[2])
+        if g["x"] is not None:
+            g["x"] = g["x"].view(x.shape[0], x.shape[1], x.shape[2], 1)
+        g["weight"] = g["weight"].view_as(ctx.owner.nn[0].weight)
+        pick = lambda i, key: g[key] if need[i] else None
+        return (None, None, pick(2, "x"), None, None, pick(5, "weight"), pick(6, "bias"), pick(7, "prelu"),
+                pick(8, "bn_weight"), pick(9, "bn_bias"))
 
 
-class _DenseGraphConv(nn.Module):
+class _DenseGraphConv(BasicConvLowering, nn.Module):
     """Shared plumbing of EdgeConv2d / MRConv2d."""
     _conv = None
 
@@ -53,58 +63,16 @@ class _DenseGraphConv(nn.Module):
             if isinstance(m, nn.InstanceNorm2d):      # unreachable in the reference as well
                 raise NotImplementedError("normalization layer [instance] is not supported by the graph convs")
 
-    def _parts(self):
-        conv, act, prelu, bn = self.nn[0], None, None, None
-        for m in list(self.nn)[1:]:
-            if isinstance(m, nn.ReLU):
-                act = "relu"
-            elif isinstance(m, nn.LeakyReLU):
-                act = "leakyrelu"
-            elif isinstance(m, nn.PReLU):
-                act, prelu = "prelu", m.weight
-            elif isinstance(m, (nn.BatchNorm2d, nn.SyncBatchNorm)):    # (convert_sync_batchnorm)
-                bn = m
-        return conv, act, prelu, bn
-
-    def _conv_params(self):
-        conv, act, prelu, bn = self._parts()
-        norm = _native.NORM_NONE
-        kw = {}
-        if bn is not None:
-            use_batch = self.training or bn.running_mean is None
-            norm = _native.NORM_BATCH_TRAIN if use_batch else _native.NORM_BATCH_EVAL
-            kw = dict(bn_weight=bn.weight, bn_bias=bn.bias, bn_mean=bn.running_mean, bn_var=bn.running_var,
-                      bn_eps=bn.eps, sync_group=_native.sync_group(bn))
-        return _native.ConvParams(conv.weight, conv.bias, act, prelu, norm, **kw)
-
-    def _after_forward(self, prm, x, out, k):
-        """BatchNorm2d training bookkeeping (running statistics, momentum, unbiased
-        variance, num_batches_tracked) exactly as torch does it.  With synced statistics the
-        variance is unbiased with the global count, read on the device."""
-        bn = self._parts()[3]
-        if bn is None or prm.norm != _native.NORM_BATCH_TRAIN or not bn.track_running_stats:
-            return
-        with torch.no_grad():
-            bn.num_batches_tracked += 1
-            mom = bn.momentum if bn.momentum is not None else 1.0 / float(bn.num_batches_tracked)
-            if prm.moments is not None:
-                count = prm.moments[-1]
-                unbiased = prm.batch_var * (count / (count - 1).clamp_min(1)).float()
-            else:
-                count = x.shape[0] * x.shape[2] * (k if self._conv == "edge" else 1)
-                unbiased = prm.batch_var * (count / max(count - 1, 1))
-            bn.running_mean.mul_(1 - mom).add_(prm.batch_mean, alpha=mom)
-            bn.running_var.mul_(1 - mom).add_(unbiased, alpha=mom)
-
     def _run(self, x, edge_index, fused=None, block=None):
-        conv, act, prelu, bn = self._parts()
+        parts = self._parts()
+        conv, act, prelu, bn = parts
         params = (conv.weight, conv.bias, prelu, None if bn is None else bn.weight, None if bn is None else bn.bias)
         if fused is not None:
             # the graph is kept (int32 neighbour list) only when a backward pass can follow
             need = torch.is_grad_enabled() and (x.requires_grad or any(
                 p is not None and p.requires_grad for p in params))
             fused = tuple(fused) + (need,) + ((block,) if block else ())
-        return _GraphConvFn.apply(self, x, edge_index, fused, *params)
+        return _GraphConvFn.apply(self, parts, x, edge_index, fused, *params)
 
     def can_fuse_block(self, x):
         """The block epilogue (skip connection / slice write in the consumer's store) runs without autograd and

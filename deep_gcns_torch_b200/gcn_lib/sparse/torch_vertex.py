@@ -5,6 +5,7 @@ import torch
 from torch import nn
 
 from ... import _native
+from .._basic_conv import BasicConvLowering, update_running_stats
 from .torch_nn import MLP, BondEncoder
 from .torch_edge import DilatedKnnGraph
 from .torch_message import GenMessagePassing, MsgNorm, _AggregateFn, csr_of
@@ -108,11 +109,11 @@ class _EdgeConvFn(torch.autograd.Function):
     """autograd node of EdgConv: dgcn_sparse_edge_conv_forward / _backward over the cached CSR graph."""
 
     @staticmethod
-    def forward(ctx, owner, csr, n_edges, x, weight, bias, prelu, bn_w, bn_b):
-        prm = owner._conv_params()
+    def forward(ctx, owner, parts, csr, n_edges, x, weight, bias, prelu, bn_w, bn_b):
+        prm = owner._conv_params(parts)
         out = _native.sparse_edge_conv_forward(x, csr, n_edges, prm)
-        owner._after_forward(prm, n_edges)
-        ctx.owner, ctx.prm, ctx.csr, ctx.n_edges = owner, prm, csr, n_edges
+        update_running_stats(parts[3], prm, n_edges)      # BatchNorm over the E edge rows
+        ctx.prm, ctx.csr, ctx.n_edges = prm, csr, n_edges
         ctx.save_for_backward(x)
         return out
 
@@ -120,13 +121,13 @@ class _EdgeConvFn(torch.autograd.Function):
     def backward(ctx, grad_out):
         (x,) = ctx.saved_tensors
         need = ctx.needs_input_grad
-        g = _native.sparse_edge_conv_backward(x, ctx.csr, ctx.n_edges, ctx.prm, grad_out, need_x=need[3])
+        g = _native.sparse_edge_conv_backward(x, ctx.csr, ctx.n_edges, ctx.prm, grad_out, need_x=need[4])
         pick = lambda i, key: g[key] if need[i] else None
-        return (None, None, None, pick(3, "x"), pick(4, "weight"), pick(5, "bias"), pick(6, "prelu"),
-                pick(7, "bn_weight"), pick(8, "bn_bias"))
+        return (None, None, None, None, pick(4, "x"), pick(5, "weight"), pick(6, "bias"), pick(7, "prelu"),
+                pick(8, "bn_weight"), pick(9, "bn_bias"))
 
 
-class EdgConv(nn.Module):
+class EdgConv(BasicConvLowering, nn.Module):
     """Edge convolution, sparse layout (torch_vertex.py:106-114, torch_geometric's EdgeConv around
     MLP([2*C_in, C_out], act, norm, bias): Linear -> norm -> act):
     out_i = max over edges (j -> i) of nn(cat[x_i, x_j - x_i]), 0 for a node without in-edges.  One CSR edge pass
@@ -144,56 +145,9 @@ class EdgConv(nn.Module):
         self.nn = MLP([in_channels * 2, out_channels], act, norm, bias)
         self.aggr = aggr
 
-    def _parts(self):
-        lin, act, prelu, bn = self.nn[0], None, None, None
-        for m in list(self.nn)[1:]:
-            if isinstance(m, nn.ReLU):
-                act = "relu"
-            elif isinstance(m, nn.LeakyReLU):
-                act = "leakyrelu"
-            elif isinstance(m, nn.PReLU):
-                act, prelu = "prelu", m.weight
-            elif isinstance(m, (nn.BatchNorm1d, nn.SyncBatchNorm)):
-                bn = m
-            else:
-                raise NotImplementedError("EdgConv: layer {} is not supported in the MLP".format(type(m).__name__))
-        if prelu is not None and prelu.numel() != 1:
-            raise NotImplementedError("EdgConv: PReLU with one weight per channel is not supported")
-        return lin, act, prelu, bn
-
-    def _conv_params(self):
-        lin, act, prelu, bn = self._parts()
-        norm, kw = _native.NORM_NONE, {}
-        if bn is not None:
-            use_batch = self.training or bn.running_mean is None
-            norm = _native.NORM_BATCH_TRAIN if use_batch else _native.NORM_BATCH_EVAL
-            kw = dict(bn_weight=bn.weight, bn_bias=bn.bias, bn_mean=bn.running_mean, bn_var=bn.running_var,
-                      bn_eps=bn.eps, sync_group=_native.sync_group(bn))
-        return _native.ConvParams(lin.weight, lin.bias, act, prelu, norm, **kw)
-
-    def _after_forward(self, prm, n_edges):
-        """BatchNorm1d training bookkeeping over the E edge rows, the rule of the dense convolutions' _after_forward
-        (momentum, unbiased variance, num_batches_tracked).  An edgeless batch leaves the running statistics as
-        torch does.  With synced statistics the variance is unbiased with the global edge count, read on the device,
-        and a rank without edges updates its running statistics from the global ones like its peers."""
-        bn = self._parts()[3]
-        if bn is None or prm.norm != _native.NORM_BATCH_TRAIN or not bn.track_running_stats:
-            return
-        with torch.no_grad():
-            bn.num_batches_tracked += 1
-            if prm.moments is None and n_edges == 0:
-                return
-            mom = bn.momentum if bn.momentum is not None else 1.0 / float(bn.num_batches_tracked)
-            if prm.moments is not None:
-                count = prm.moments[-1]
-                unbiased = prm.batch_var * (count / (count - 1).clamp_min(1)).float()
-            else:
-                unbiased = prm.batch_var * (n_edges / max(n_edges - 1, 1))
-            bn.running_mean.mul_(1 - mom).add_(prm.batch_mean, alpha=mom)
-            bn.running_var.mul_(1 - mom).add_(unbiased, alpha=mom)
-
     def forward(self, x, edge_index):
-        lin, act, prelu, bn = self._parts()
+        parts = self._parts()
+        lin, act, prelu, bn = parts
         if isinstance(bn, nn.SyncBatchNorm) and not (x.is_cuda and edge_index.is_cuda):
             raise NotImplementedError("EdgConv: the sparse EdgeConv's SyncBatchNorm needs CUDA tensors")
         _native._require_cuda(x, edge_index)
@@ -206,7 +160,7 @@ class EdgConv(nn.Module):
             raise ValueError("Expected more than 1 value per channel when training, got input size %s"
                              % (torch.Size([1, lin.out_features]),))       # what BatchNorm1d raises
         csr = csr_of(edge_index, x.size(0))
-        return _EdgeConvFn.apply(self, csr, n_edges, x, lin.weight, lin.bias, prelu,
+        return _EdgeConvFn.apply(self, parts, csr, n_edges, x, lin.weight, lin.bias, prelu,
                                  None if bn is None else bn.weight, None if bn is None else bn.bias)
 
 

@@ -208,7 +208,9 @@ int dgcn_dyn_conv_forward(int32_t conv, const float* x, int64_t B, int64_t C_in,
  * grad_x is (B, C_in, N) contiguous.
  * grad_weight (C_out,2*C_in), grad_bias (C_out), grad_bn_weight/bias (C_out),
  * grad_prelu (1) are OVERWRITTEN; any of them may be NULL.
- * sync: dgcn_bn_sync or NULL. */
+ * sync: dgcn_bn_sync or NULL.
+ * An act or norm out of range is DGCN_ERR_UNSUPPORTED and a PReLU without prelu_weight DGCN_ERR_BAD_ARG, as in
+ * the forward. */
 size_t dgcn_graph_conv_backward_workspace_bytes(int32_t conv, int64_t B, int64_t C_in,
                                                 int64_t C_out, int64_t N, int64_t k);
 int dgcn_graph_conv_backward(int32_t conv, const float* x, int64_t B, int64_t C_in, int64_t N,

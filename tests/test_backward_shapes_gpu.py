@@ -5,7 +5,7 @@ Every case checks the forward output and every gradient the layer has, elementwi
 upstream gradient at the near-ties of the max (at most 1e-3 of the entries); MRConv cases use seeds without
 near-ties.  Each case prints its worst |got - ref| / max|ref| per gradient and the masked fraction.
 
-dense_bwd.cu paths, and the case that reaches each:
+Paths of dgcn_graph_conv_backward (dense_bwd.cu, its GEMMs in basic_conv.cu), and the case that reaches each:
   wgrad_kernel over several KCH = 512 chunks with a partial last one     a (2 chunks), c (8), d (3, 6-point tail)
   tile_gemm_kernel / wgrad_kernel over several 128-wide tiles              d (C_in 130 / 160, 2 C_out = 192)
   unaligned operands (ci % 4 != 0, vec = 0, N % 4 != 0)                   b (C_in 3, N 1030, misaligned x), d

@@ -1,5 +1,5 @@
 """CPU restatement of the dense path's train-mode BatchNorm statistics (common.cuh: bn_acc_add, bn_acc_moments,
-bn_merge; dense_fwd.cu: bn_merge_kernel), fp32 emulated with np.float32, in the kernels' order:
+bn_merge; basic_conv.cu: bn_merge_kernel), fp32 emulated with np.float32, in the kernels' order:
 
 - each thread sums a - pivot and (a - pivot)^2 along its chain (pivot = its first value),
 - threads of a warp merge (count, mean, M2) with Chan's formula along an xor-shuffle tree, warps in order,

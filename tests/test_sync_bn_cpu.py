@@ -97,6 +97,20 @@ def test_dense_parts_see_sync_batchnorm():
     assert m.gconv._conv_params().sync_group is None
 
 
+def test_dense_parts_reject_layers_the_kernels_do_not_run():
+    """A BasicConv edited to hold a layer the fused kernels do not run raises instead of running without it, by the
+    rule of the sparse EdgConv's MLP."""
+    from deep_gcns_torch_b200.gcn_lib import dense as D
+    conv = D.EdgeConv2d(4, 8, "relu", "batch")
+    conv.nn.append(nn.Dropout2d(0.5))
+    with pytest.raises(NotImplementedError, match="Dropout2d"):
+        conv(torch.randn(1, 4, 16, 1), torch.zeros((2, 1, 16, 3), dtype=torch.long))
+    conv = D.MRConv2d(4, 8, "prelu")
+    conv.nn[1] = nn.PReLU(8)
+    with pytest.raises(NotImplementedError, match="PReLU"):
+        conv._parts()
+
+
 def test_sparse_fused_block_accepts_eval_sync_batchnorm():
     from deep_gcns_torch_b200.gcn_lib import sparse as S
     from deep_gcns_torch_b200.gcn_lib.sparse.fused import fusable

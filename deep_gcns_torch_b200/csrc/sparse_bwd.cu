@@ -37,6 +37,15 @@ template <> __device__ __forceinline__ float from_f32<float>(float v) { return v
 template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
 template <> __device__ __forceinline__ __half from_f32<__half>(float v) { return __float2half_rn(v); }
 
+// s += v with the rounding error carried in c (Kahan).  Pass A sums a whole row in one fp32 chain per lane; on a row
+// of 10^6 edges a plain chain leaves the softmax sum S ~3e-3 off, and every weight e / S with it.
+__device__ __forceinline__ void kahan_add(float& s, float& c, float v) {
+  const float y = v - c;
+  const float sum = s + y;
+  c = (sum - s) - y;
+  s = sum;
+}
+
 // T: element type of the rows (float, __nv_bfloat16, __half); NCH: channels per lane (c = lane + 32*u, so channel
 // c's keep bit is bit `lane` of the row's word u); PRE: the forward's pre-activation (+ keep mask), fp32 rows.
 template <typename T, int NCH, bool PRE = false>
@@ -70,10 +79,12 @@ __global__ void __launch_bounds__(256) genconv_aggregate_bwd_kernel(const AggrBw
 
   // ---- pass A: recompute the aggregate ---------------------------------------------------------
   float M[NCH], S[NCH], W[NCH], L[NCH];   // running max, sum exp / count, weighted sum, sum u^p ln u
+  float cS[NCH], cW[NCH];                 // softmax: Kahan compensations of S and W
   int arg[NCH];
 #pragma unroll
   for (int u = 0; u < NCH; ++u) {
     M[u] = -INFINITY; S[u] = 0.f; W[u] = (aggr == DGCN_AGGR_MAX) ? -INFINITY : 0.f; L[u] = 0.f; arg[u] = -1;
+    cS[u] = 0.f; cW[u] = 0.f;
   }
   for (int e = beg; e < end; ++e) {
     const int s = __ldg(g.src + e);
@@ -87,8 +98,15 @@ __global__ void __launch_bounds__(256) genconv_aggregate_bwd_kernel(const AggrBw
         const float msg = g.raw ? v : fmaxf(v, 0.f) + g.eps;
         if (softmax) {
           const float z = msg * t, d = z - M[u], ex = __expf(-fabsf(d));
-          if (d > 0.f) { S[u] = fmaf(S[u], ex, 1.f); W[u] = fmaf(W[u], ex, msg); M[u] = z; }
-          else { S[u] += ex; W[u] = fmaf(ex, msg, W[u]); }
+          if (d > 0.f) {   // new running max: rescale the sums with their compensations, then add this edge
+            S[u] *= ex; cS[u] *= ex; W[u] *= ex; cW[u] *= ex;
+            kahan_add(S[u], cS[u], 1.f);
+            kahan_add(W[u], cW[u], msg);
+            M[u] = z;
+          } else {
+            kahan_add(S[u], cS[u], ex);
+            kahan_add(W[u], cW[u], ex * msg);
+          }
         } else if (power) {
           const float uu = fminf(fmaxf(msg, 1e-7f), 10.f);
           const float up = __powf(uu, p);

@@ -4,6 +4,7 @@ import pytest
 import torch
 
 import golden_util as gu
+import ogb_graph_util as ogb
 from oracle import sparse as osp
 
 pytestmark = pytest.mark.gpu
@@ -36,17 +37,38 @@ def test_golden_genconv(name):
         torch.testing.assert_close(mod.sigmoid_y.cpu(), torch.sigmoid(c.sd["y"]))
 
 
+def _first_diff(got, want):
+    i = int((got != want).nonzero()[0, 0])
+    return "first difference at %d: got %d, want %d" % (i, int(got[i]), int(want[i]))
+
+
 def test_csr_build_is_stable_and_complete():
+    """dgcn_csr_build against a stable sort of the destinations on the device.  Besides small and empty graphs:
+    - the ogbn-products shape (N = 2,449,029, E = 61,859,140): the radix histogram has 256 * ceil(E / RS_CHUNK)
+      > 2^20 entries and rowptr N + 1 > 2^20, so scan_totals_kernel scans several 1024-block strips and carries
+      between them (8 strips for the histogram, 3 for rowptr);
+    - N = 2^24 + 5: destinations need 25 bits, so the sort makes 4 passes, N - 1 included."""
     from deep_gcns_torch_b200 import _native
-    g = torch.Generator().manual_seed(0)
-    for (n, e) in [(1, 5), (10, 0), (300, 3050), (70000, 200000), (5, 4099)]:
-        ei = torch.stack((torch.randint(0, n, (e,), generator=g), torch.randint(0, n, (e,), generator=g)))
-        rowptr, src, eid = _native.csr_build(ei.cuda(), n)[:3]
+    g = torch.Generator(device="cuda").manual_seed(0)
+    for (n, e) in [(1, 5), (10, 0), (300, 3050), (70000, 200000), (5, 4099), ogb.PRODUCTS, (2**24 + 5, 4_000_000)]:
+        if (n, e) == ogb.PRODUCTS:
+            ei = ogb.products_edges()
+            assert 256 * ogb.ceil_div(e, ogb.RS_CHUNK) > 2**20 and n + 1 > 2**20
+        else:
+            ei = torch.randint(0, n, (2, e), generator=g, device="cuda")
+        if n > 2**24:
+            ei[1, ::4001] = n - 1
+            assert ogb.radix_passes(n) == 4 and int(ei[1].max()) == n - 1
+        rowptr, src, eid = _native.csr_build(ei, n)[:3]
         order = torch.sort(ei[1], stable=True).indices
-        assert torch.equal(eid.cpu().long()[:e], order)
-        assert torch.equal(src.cpu().long()[:e], ei[0][order])
-        deg = torch.bincount(ei[1], minlength=n)
-        assert torch.equal(rowptr.cpu().long(), torch.cat([torch.zeros(1, dtype=torch.long), deg.cumsum(0)]))
+        what = "csr_build N=%d E=%d, " % (n, e)
+        assert torch.equal(eid[:e].long(), order), what + "eid " + _first_diff(eid[:e].long(), order)
+        want_src = ei[0][order]
+        assert torch.equal(src[:e].long(), want_src), what + "src " + _first_diff(src[:e].long(), want_src)
+        want_ptr = torch.cat((torch.zeros(1, dtype=torch.long, device="cuda"), torch.bincount(ei[1], minlength=n).cumsum(0)))
+        assert torch.equal(rowptr.long(), want_ptr), what + "rowptr " + _first_diff(rowptr.long(), want_ptr)
+        del ei, rowptr, src, eid, order, want_src, want_ptr
+        torch.cuda.empty_cache()
 
 
 AGGRS = ["softmax", "softmax_sg", "softmax_sum", "power", "power_sum", "add", "mean", "max"]
@@ -243,34 +265,50 @@ def test_partitioned_layer_emulated_on_one_gpu():
     assert parts[0].interior_rows.numel() > 0 and parts[0].boundary_rows.numel() > 0
 
 
-@pytest.mark.parametrize("N,K,M", [(1000, 128, 128), (129, 64, 32), (5000, 256, 64), (3000, 64, 256), (128 * 150 + 7, 128, 64), (1, 64, 96)])
-def test_tcgen05_row_linear_with_bias_and_skip(N, K, M):
+@pytest.mark.parametrize("N,K,M", [
+    (1000, 128, 128), (129, 64, 32), (5000, 256, 64), (3000, 64, 256), (128 * 150 + 7, 128, 64), (1, 64, 96),
+    (20000, 256, 96),                     # at K = 256 the widest M whose W and A planes fit one SM's shared memory
+    (5000, 128, 160), (5000, 64, 224),    # odd numbers of 32-column output blocks
+    (132534, 64, 64),                     # ogbn-proteins' hidden width: ~8 tiles per CTA
+    (169343, 128, 128),                   # ogbn-arxiv: ~10 tiles per CTA
+    (2449029, 128, 128),                  # ogbn-products: ~145 tiles per CTA
+])
+def test_row_linear_with_bias_and_skip(N, K, M):
     """dgcn_linear_residual (wgmma, two-plane bf16 split of both operands) against an fp64 Linear: the split
     leaves <= ~2^-16 * sum|a||w| of error, far inside the 1e-3 parity tolerance; bias / skip optional; rows beyond
-    the last full 128-row tile; out aliasing res."""
+    the last full 128-row tile; out aliasing res.  The OGB row counts run the persistent tile loop for 3 and more
+    tiles per CTA, where the a_full / a_free mbarrier phases wrap around.  The fp64 reference is taken in row chunks."""
     from deep_gcns_torch_b200 import _native
-    g = torch.Generator().manual_seed(N + K + M)
-    a = (torch.randn(N, K, generator=g) * 3).cuda()
-    w = torch.randn(M, K, generator=g).cuda() / K ** 0.5
-    b = torch.randn(M, generator=g).cuda()
-    h = torch.randn(N, M, generator=g).cuda()
-    mag = a.double().abs() @ w.double().abs().t()                      # sum_k |a||w| per output
+    g = torch.Generator(device="cuda").manual_seed(N + K + M)
+    a = torch.randn(N, K, generator=g, device="cuda") * 3
+    w = torch.randn(M, K, generator=g, device="cuda") / K ** 0.5
+    b = torch.randn(M, generator=g, device="cuda")
+    h = torch.randn(N, M, generator=g, device="cuda")
+    if N >= 100000:
+        assert -(-N // 128) > 2 * torch.cuda.get_device_properties(0).multi_processor_count   # a third tile per CTA
+    w64 = w.double()
+
+    def check(out, bias, res, chunk=1 << 17):
+        for lo in range(0, N, chunk):
+            a64 = a[lo:lo + chunk].double()
+            ref = a64 @ w64.t()
+            mag = a64.abs() @ w64.abs().t()                            # sum_k |a||w| per output
+            if bias is not None:
+                ref = ref + bias.double()
+            if res is not None:
+                ref = ref + res[lo:lo + chunk].double()
+            got = out[lo:lo + chunk]
+            err = (got.double() - ref).abs()
+            assert bool((err <= 4e-5 * mag + 1e-6 * ref.abs() + 1e-6).all()), (lo, float((err / (mag + 1e-9)).max()))
+            torch.testing.assert_close(got, ref.float(), rtol=1e-3, atol=1e-4)
+
     for bias, res in ((b, h), (None, h), (b, None), (None, None)):
-        ref = a.double() @ w.double().t()
-        if bias is not None:
-            ref = ref + bias.double()
-        if res is not None:
-            ref = ref + res.double()
-        out = _native.linear_residual(a, w, bias, res)
-        err = (out.double() - ref).abs()
-        assert bool((err <= 4e-5 * mag + 1e-6 * ref.abs() + 1e-6).all()), float((err / (mag + 1e-9)).max())
-        torch.testing.assert_close(out, ref.float(), rtol=1e-3, atol=1e-4)
+        check(_native.linear_residual(a, w, bias, res), bias, res)
     b_odd = torch.cat((torch.zeros(1, device="cuda"), b))[1:]            # bias at an odd float offset (4-byte aligned)
-    torch.testing.assert_close(_native.linear_residual(a, w, b_odd, h),
-                               (a.double() @ w.double().t() + b.double() + h.double()).float(), rtol=1e-3, atol=1e-4)
+    check(_native.linear_residual(a, w, b_odd, h), b, h)
     buf = h.clone()
     _native.linear_residual(a, w, b, buf, out=buf)                     # in place on the skip tensor
-    torch.testing.assert_close(buf, (a.double() @ w.double().t() + b.double() + h.double()).float(), rtol=1e-3, atol=1e-4)
+    check(buf, b, h)
     assert not _native.linear_residual_supported(100, 128) and not _native.linear_residual_supported(128, 300)
     assert not _native.linear_residual_supported(256, 256)            # operands would not fit one SM's shared memory
 

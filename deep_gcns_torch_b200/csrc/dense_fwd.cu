@@ -201,43 +201,6 @@ static cudaStream_t slab_side_stream() {
   return s;
 }
 
-// cuTensorMapEncodeTiled through the runtime (no link against libcuda): resolved once, the pointer is a
-// write-once cache of a driver symbol.
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn tensor_map_encoder() {
-  static std::atomic<void*> cached{nullptr};
-  void* fn = cached.load(std::memory_order_acquire);
-  if (!fn) {
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess)
-      return nullptr;
-    cached.store(fn, std::memory_order_release);
-  }
-  return reinterpret_cast<EncodeTiledFn>(fn);
-}
-// 16-bit matrix (rows, cols) row-major, elements of type `dtype` (bf16 or fp16) -> tensor map with boxes of box_cols
-// columns x box_rows rows.  box_cols = 64 (128 bytes), SWIZZLE_128B: a box lands in shared memory as box_rows x 128 B
-// rows with the 16-byte chunks XOR-swizzled by (row & 7), which is the canonical MN-major wgmma layout of one 64-wide
-// MN block; box_cols = 32 (64 bytes), SWIZZLE_64B: box_rows x 64 B rows, chunks XOR-swizzled by ((row >> 1) & 3), the
-// canonical layout of one 32-wide MN block.
-static int make_plane_map(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int box_cols, int box_rows,
-                          CUtensorMapDataType dtype) {
-  EncodeTiledFn enc = tensor_map_encoder();
-  if (!enc) return DGCN_ERR_UNSUPPORTED;
-  const cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
-  const cuuint64_t strides[1] = {static_cast<cuuint64_t>(cols) * 2};
-  const cuuint32_t box[2] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows)};
-  const cuuint32_t estr[2] = {1u, 1u};
-  const CUtensorMapSwizzle swz = box_cols == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
-  const CUresult rc = enc(map, dtype, 2, const_cast<void*>(base), dims, strides, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return rc == CUDA_SUCCESS ? DGCN_OK : DGCN_ERR_CUDA;
-}
-
 // Tensor-core pre-filter route (knn_tc.cuh).
 static int launch_knn_tc(KnnArgs& a, const KnnPlan& pl, const KnnRegions& r, cudaStream_t stream,
                          const ProloguePq* pqf) {
@@ -265,16 +228,16 @@ static int launch_knn_tc(KnnArgs& a, const KnnPlan& pl, const KnnRegions& r, cud
   DGCN_LAUNCH_CHECK();
   TcArgs t{};
   {
-    int rc = quad ? make_plane_map(&t.tm_planes, r.planes, static_cast<int64_t>(B) * cpad, N, 64, cpad,
-                                   CU_TENSOR_MAP_DATA_TYPE_FLOAT16)
-                  : make_plane_map(&t.tm_planes, r.planes, static_cast<int64_t>(B) * TC_PLANES * cpad, N, 64, cpad,
-                                   CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
+    int rc = quad ? make_tensor_map(&t.tm_planes, r.planes, static_cast<int64_t>(B) * cpad, N, 64, cpad,
+                                    CU_TENSOR_MAP_DATA_TYPE_FLOAT16)
+                  : make_tensor_map(&t.tm_planes, r.planes, static_cast<int64_t>(B) * TC_PLANES * cpad, N, 64, cpad,
+                                    CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
     if (rc == DGCN_OK)
-      rc = make_plane_map(&t.tm_sqp, r.sqp, static_cast<int64_t>(B) * 8, N, 64, 8, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
+      rc = make_tensor_map(&t.tm_sqp, r.sqp, static_cast<int64_t>(B) * 8, N, 64, 8, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
     if (quad && rc == DGCN_OK)   // knn_tc4_kernel's 32-candidate tiles
-      rc = make_plane_map(&t.tm_cand, r.planes, static_cast<int64_t>(B) * cpad, N, T4_CT, cpad, CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
+      rc = make_tensor_map(&t.tm_cand, r.planes, static_cast<int64_t>(B) * cpad, N, T4_CT, cpad, CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
     if (quad && rc == DGCN_OK)
-      rc = make_plane_map(&t.tm_sqc, r.sqp, static_cast<int64_t>(B) * 8, N, T4_CT, 8, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
+      rc = make_tensor_map(&t.tm_sqc, r.sqp, static_cast<int64_t>(B) * 8, N, T4_CT, 8, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
     if (rc != DGCN_OK) return rc;
   }
   t.a = a;

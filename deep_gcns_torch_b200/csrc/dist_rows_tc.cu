@@ -20,11 +20,10 @@
 // canonical MN-major wgmma layout, like knn_tc): the TMA of tile t+2 runs under the wgmma and epilogue of tile t+1.
 // Epilogue: each quad of lanes stores 8 consecutive floats (one 32-byte sector) of a row of
 // (sq_i + (-2 acc)) + sq_j.
-#include <cuda.h>
 #include <cuda_bf16.h>
 
-#define DGCN_TEMPLATES_ONLY      // device helpers of knn_tc.cuh only: its kernels live in dense_fwd.cu
 #include "knn_tc.cuh"
+#include "tma.cuh"
 #include "wgmma.cuh"
 
 namespace dgcn {
@@ -82,13 +81,13 @@ __global__ void __launch_bounds__(288, 1) dist_rows_tc_kernel(const __grid_const
   const int tile0 = static_cast<int>(blockIdx.y) * ntiles;              // first of them
   const int plane_bytes = 2 * Cpad * 128;
   if (tid == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&g.tm_planes)) : "memory");
+    prefetch_tensormap(&g.tm_planes);
     mbar_init(&bar.q_full, 1);
     for (int i = 0; i < 2; ++i) {
       mbar_init(&bar.tma_full[i], 1);
       mbar_init(&bar.stage_free[i], 256);
     }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init_fence();
   }
   if (tid < TILE) sqq_s[tid] = __ldg(g.sq + static_cast<int64_t>(b) * N + q0 + tid);
   __syncthreads();
@@ -157,22 +156,6 @@ __global__ void __launch_bounds__(288, 1) dist_rows_tc_kernel(const __grid_const
   }
 }
 
-typedef CUresult (*DrEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static DrEncodeFn dr_encoder() {
-  static std::atomic<void*> cached{nullptr};
-  void* fn = cached.load(std::memory_order_acquire);
-  if (!fn) {
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess)
-      return nullptr;
-    cached.store(fn, std::memory_order_release);
-  }
-  return reinterpret_cast<DrEncodeFn>(fn);
-}
-
 bool dist_rows_tc_ok(const KnnArgs& a) {
   return !a.exact_fp32 && a.C <= TC_MAX_C && a.N >= TILE && (a.N % TILE) == 0;
 }
@@ -193,27 +176,16 @@ int dist_rows_tc_prepare(const KnnArgs& a, __nv_bfloat16* planes, cudaStream_t s
 // distance rows of clouds [b0, b0 + nb) into the slab
 int dist_rows_tc_launch(const KnnArgs& a, const __nv_bfloat16* planes, int b0, int nb, float* drows, int ldd,
                         cudaStream_t stream) {
-  DrEncodeFn enc = dr_encoder();
-  if (!enc) return DGCN_ERR_UNSUPPORTED;
   const int cpad = (a.C + 15) / 16 * 16;
   DrArgs g{};
-  {
-    const cuuint64_t dims[2] = {static_cast<cuuint64_t>(a.N), static_cast<cuuint64_t>(a.B) * DR_PLANES * cpad};
-    const cuuint64_t strides[1] = {static_cast<cuuint64_t>(a.N) * 2};
-    const cuuint32_t box[2] = {64u, static_cast<cuuint32_t>(cpad)};
-    const cuuint32_t estr[2] = {1u, 1u};
-    if (enc(&g.tm_planes, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<__nv_bfloat16*>(planes), dims, strides, box, estr,
-            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return DGCN_ERR_CUDA;
-  }
+  const int rc = make_tensor_map(&g.tm_planes, planes, static_cast<int64_t>(a.B) * DR_PLANES * cpad, a.N, 64, cpad,
+                                 CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
+  if (rc != DGCN_OK) return rc;
   g.sq = a.sq; g.drows = drows; g.b0 = b0; g.N = a.N; g.Cpad = cpad; g.ldd = ldd;
   const size_t smem = static_cast<size_t>(3) * DR_PLANES * DR_PLANE_BYTES + TILE * 4 + sizeof(DrBars) + 1024;
   DGCN_ENSURE_SMEM((dist_rows_tc_kernel), smem);
   // split the candidate tiles of a query tile over CTAs until one launch fills the SMs (one CTA per SM: 146 KB smem)
-  int dev = 0, sms = 0;
-  DGCN_CUDA_TRY(cudaGetDevice(&dev));
-  DGCN_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const int sms = device_sm_count();
   const int ntiles = a.N / TILE;
   int split = 1;
   while (split * 2 <= ntiles && ntiles % (split * 2) == 0 && static_cast<int64_t>(ntiles) * nb * split * 2 <= sms) split *= 2;

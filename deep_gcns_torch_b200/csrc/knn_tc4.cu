@@ -1,6 +1,5 @@
 // knn_tc4_kernel<20 / 32>: the multi-tile, warp-specialised tensor-core selection (knn_tc4.cuh) in its own
 // translation unit (long ptxas runs of the sorting networks compile in parallel with the other kernels).
-#define DGCN_TEMPLATES_ONLY
 #include "knn_tc4.cuh"
 
 namespace dgcn {

@@ -145,15 +145,15 @@ __global__ void __launch_bounds__(T4_THREADS, 1) knn_tc4_kernel(const __grid_con
   const int plane_q = 2 * Cpad * 128, plane_c = Cpad * 64;                // fp16 query plane / candidate tile
 
   if (tid == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&t.tm_planes)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&t.tm_cand)) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&t.tm_sqc)) : "memory");
+    prefetch_tensormap(&t.tm_planes);
+    prefetch_tensormap(&t.tm_cand);
+    prefetch_tensormap(&t.tm_sqc);
     for (int s = 0; s < T4_STAGES; ++s) {
       mbar_init(&sm.full[s], 1);
       mbar_init(&sm.stage_free[s], static_cast<uint32_t>(ngroups * 128));
     }
     mbar_init(&sm.q_full, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init_fence();
   }
   // constant operand blocks: ones in K rows 0..2 on the query side; the candidate-side blocks are zero in rows
   // 8..15 (TMA refreshes rows 0..7 of a stage with every tile).  Whole rows are constant: no swizzle needed.

@@ -1,6 +1,5 @@
 // knn_tc_kernel<16, packed / unpacked>: one translation unit per list length so that the long ptxas runs
 // of the register-resident insertion networks compile in parallel.
-#define DGCN_TEMPLATES_ONLY
 #include "knn_tc.cuh"
 
 namespace dgcn {

@@ -21,10 +21,10 @@
 //                          epilogue -, then out = acc + bias + res straight from the accumulator fragments (each quad
 //                          of lanes covers 8 consecutive floats = one 32-byte sector of a row).
 //   W (hi, mid)            resident in shared memory for the life of the CTA, loaded once by TMA.
-#include <cuda.h>
 #include <cuda_bf16.h>
 
 #include "common.cuh"
+#include "tma.cuh"
 #include "wgmma.cuh"
 
 namespace dgcn {
@@ -32,39 +32,6 @@ namespace dgcn {
 constexpr int RL_TILE = 128;          // rows per tile = MMA M
 constexpr int RL_MAX = 256;           // K and M upper bound
 
-__device__ __forceinline__ uint32_t rl_smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-__device__ __forceinline__ void rl_mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(rl_smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void rl_mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(rl_smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void rl_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(rl_smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void rl_mbar_wait(uint64_t* bar, uint32_t parity) {
-  for (uint32_t spin = 0;; ++spin) {   // bounded: a pipeline that never signals must trap, not hang the GPU
-    uint32_t done;
-    asm volatile(
-        "{\n"
-        ".reg .pred P1;\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 P1, [%1], %2;\n"
-        "selp.u32 %0, 1, 0, P1;\n"
-        "}"
-        : "=r"(done)
-        : "r"(rl_smem_u32(bar)), "r"(parity)
-        : "memory");
-    if (done) return;
-    if (spin > (1u << 26)) __trap();
-  }
-}
-__device__ __forceinline__ void rl_tma_load_2d(uint32_t smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-          smem_dst),
-      "l"(reinterpret_cast<uint64_t>(map)), "r"(rl_smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
 // W (M,K) fp32 -> Wp (2, M, K) bf16 (hi, mid)
 __global__ void rl_split_weights_kernel(const float* __restrict__ w, int64_t n, __nv_bfloat16* __restrict__ wp) {
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -96,7 +63,7 @@ constexpr int RL_NB = RL_MAX / 32;    // 32-column output blocks
 
 __global__ void __launch_bounds__(RL_EPI_THREADS + 128, 1) rowlinear_tc_kernel(const __grid_constant__ RlArgs g) {
   extern __shared__ __align__(16) unsigned char rl_smem[];
-  unsigned char* base = rl_smem + ((1024u - (rl_smem_u32(rl_smem) & 1023u)) & 1023u);
+  unsigned char* base = rl_smem + ((1024u - (smem_u32(rl_smem) & 1023u)) & 1023u);
   const int K = g.K, M = g.M;
   const int kblocks = K / 64;
   const uint32_t w_plane = static_cast<uint32_t>(M) * K * 2;            // bytes of one W plane
@@ -108,10 +75,10 @@ __global__ void __launch_bounds__(RL_EPI_THREADS + 128, 1) rowlinear_tc_kernel(c
   const int64_t ntiles = (g.N + RL_TILE - 1) / RL_TILE;
 
   if (tid == 0) {
-    rl_mbar_init(&bar.w_full, 1);
-    rl_mbar_init(&bar.a_full, 128);
-    rl_mbar_init(&bar.a_free, RL_EPI_THREADS);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    mbar_init(&bar.w_full, 1);
+    mbar_init(&bar.a_full, 128);
+    mbar_init(&bar.a_free, RL_EPI_THREADS);
+    mbar_init_fence();
   }
   __syncthreads();
 
@@ -119,10 +86,10 @@ __global__ void __launch_bounds__(RL_EPI_THREADS + 128, 1) rowlinear_tc_kernel(c
     // ======================= producers ===============================================================================
     const int pt = tid - RL_EPI_THREADS;
     if (pt == 0) {   // W: one box of 64 k x M rows per (plane, k-block)
-      rl_mbar_expect_tx(&bar.w_full, 2 * w_plane);
+      mbar_expect_tx(&bar.w_full, 2 * w_plane);
       for (int pl = 0; pl < 2; ++pl)
         for (int kb = 0; kb < kblocks; ++kb)
-          rl_tma_load_2d(rl_smem_u32(w_s) + pl * w_plane + kb * (M * 128), &g.tm_w, kb * 64, pl * M, &bar.w_full);
+          tma_load_2d(smem_u32(w_s) + pl * w_plane + kb * (M * 128), &g.tm_w, kb * 64, pl * M, &bar.w_full);
     }
     const int chunks = K / 8;                       // 16-byte bf16 chunks per row
     const int rows_per_pass = 128 / chunks;         // K = 64: 16 rows, 128: 8 rows, 256: 4 rows
@@ -148,7 +115,7 @@ __global__ void __launch_bounds__(RL_EPI_THREADS + 128, 1) rowlinear_tc_kernel(c
           }
         }
         // the A buffer is still read by the previous tile's wgmma: wait only now, with this tile's first loads in flight
-        if (r0 == 0 && it > 0) rl_mbar_wait(&bar.a_free, static_cast<uint32_t>((it - 1) & 1));
+        if (r0 == 0 && it > 0) mbar_wait(&bar.a_free, static_cast<uint32_t>((it - 1) & 1));
 #pragma unroll
         for (int p8 = 0; p8 < 8; ++p8) {
           const int row = r0 + p8 * rows_per_pass + rsub;
@@ -168,19 +135,19 @@ __global__ void __launch_bounds__(RL_EPI_THREADS + 128, 1) rowlinear_tc_kernel(c
           *reinterpret_cast<uint4*>(dst + a_plane) = make_uint4(pm[0], pm[1], pm[2], pm[3]);
         }
       }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");       // my generic-proxy stores -> tensor-core reads
-      rl_mbar_arrive(&bar.a_full);
+      fence_proxy_async();                                                 // my generic-proxy stores -> tensor-core reads
+      mbar_arrive(&bar.a_full);
     }
   } else {
     // ======================= consumers: wgmma, then out = acc + bias + res ==========================================
     const int wg = warp >> 2;
     const int nb = M / 32;
-    const uint32_t a_base = rl_smem_u32(a_s) + static_cast<uint32_t>(wg) * (64 * 128);   // rows 64 wg .. of every k-block
-    const uint32_t w_base = rl_smem_u32(w_s);
+    const uint32_t a_base = smem_u32(a_s) + static_cast<uint32_t>(wg) * (64 * 128);   // rows 64 wg .. of every k-block
+    const uint32_t w_base = smem_u32(w_s);
     int64_t it = 0;
     for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      if (it == 0) rl_mbar_wait(&bar.w_full, 0u);
-      rl_mbar_wait(&bar.a_full, static_cast<uint32_t>(it & 1));
+      if (it == 0) mbar_wait(&bar.w_full, 0u);
+      mbar_wait(&bar.a_full, static_cast<uint32_t>(it & 1));
       float d[RL_NB][16];
       wg_fence();
 #pragma unroll
@@ -201,7 +168,7 @@ __global__ void __launch_bounds__(RL_EPI_THREADS + 128, 1) rowlinear_tc_kernel(c
       }
       wg_commit();
       wg_wait_all();
-      rl_mbar_arrive(&bar.a_free);
+      mbar_arrive(&bar.a_free);
       const int64_t rbase = tile * RL_TILE + wg * 64;
 #pragma unroll
       for (int j = 0; j < RL_NB; ++j) {
@@ -228,22 +195,6 @@ __global__ void __launch_bounds__(RL_EPI_THREADS + 128, 1) rowlinear_tc_kernel(c
       }
     }
   }
-}
-
-typedef CUresult (*RlEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static RlEncodeFn rl_encoder() {
-  static std::atomic<void*> cached{nullptr};
-  void* fn = cached.load(std::memory_order_acquire);
-  if (!fn) {
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess)
-      return nullptr;
-    cached.store(fn, std::memory_order_release);
-  }
-  return reinterpret_cast<RlEncodeFn>(fn);
 }
 
 static size_t rl_smem_bytes(int64_t K, int64_t M) {
@@ -275,26 +226,15 @@ int dgcn_linear_residual(const float* a, int64_t N, int64_t K, const float* weig
   Workspace ws(wsp, ws_bytes);
   __nv_bfloat16* wp = ws.take<__nv_bfloat16>(static_cast<size_t>(2) * M * K);
   if (!ws.ok) return DGCN_ERR_WORKSPACE;
-  RlEncodeFn enc = rl_encoder();
-  if (!enc) return DGCN_ERR_UNSUPPORTED;
+  RlArgs g{};
+  const int rc = make_tensor_map(&g.tm_w, wp, 2 * M, K, 64, static_cast<int>(M), CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
+  if (rc != DGCN_OK) return rc;
   rl_split_weights_kernel<<<static_cast<unsigned>(ceil_div(M * K, 256)), 256, 0, stream>>>(weight, M * K, wp);
   DGCN_LAUNCH_CHECK();
-  RlArgs g{};
-  {
-    const cuuint64_t dims[2] = {static_cast<cuuint64_t>(K), static_cast<cuuint64_t>(2 * M)};
-    const cuuint64_t strides[1] = {static_cast<cuuint64_t>(K) * 2};
-    const cuuint32_t box[2] = {64u, static_cast<cuuint32_t>(M)};
-    const cuuint32_t estr[2] = {1u, 1u};
-    if (enc(&g.tm_w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, wp, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return DGCN_ERR_CUDA;
-  }
   g.a = a; g.bias = bias; g.res = res; g.out = out; g.N = N; g.K = static_cast<int>(K); g.M = static_cast<int>(M);
   const size_t smem = rl_smem_bytes(K, M);
   DGCN_ENSURE_SMEM((rowlinear_tc_kernel), smem);
-  int dev = 0, sms = 0;
-  DGCN_CUDA_TRY(cudaGetDevice(&dev));
-  DGCN_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const int sms = device_sm_count();
   const int64_t ntiles = ceil_div(N, RL_TILE);
   const unsigned grid = static_cast<unsigned>(ntiles < sms ? ntiles : sms);
   {

@@ -1,10 +1,12 @@
-// Status strings, version and per-thread CUDA error text for the dgcn C ABI.
+// Status strings, version and per-thread CUDA error text for the dgcn C ABI; the device queries and the tensor-map
+// encoder the kernels' host code shares.
 #include <stdio.h>
 #include <atomic>
 #include <mutex>
 #include <string>
 #include <vector>
 #include "common.cuh"
+#include "tma.cuh"
 
 namespace dgcn {
 static thread_local char g_last_error[512] = "";
@@ -30,6 +32,34 @@ int device_sm_count() {
 size_t device_l2_bytes() {
   static std::atomic<int> cache[64];
   return static_cast<size_t>(device_attr(cudaDevAttrL2CacheSize, cache, 50 << 20));
+}
+
+// cuTensorMapEncodeTiled through the runtime (no link against libcuda): resolved once, the pointer is a
+// write-once cache of a driver symbol.
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+int make_tensor_map(CUtensorMap* map, const void* base, int64_t rows, int64_t cols, int box_cols, int box_rows,
+                    CUtensorMapDataType dtype) {
+  static std::atomic<void*> cached{nullptr};
+  void* fn = cached.load(std::memory_order_acquire);
+  if (!fn) {
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess ||
+        q != cudaDriverEntryPointSuccess)
+      return DGCN_ERR_UNSUPPORTED;
+    cached.store(fn, std::memory_order_release);
+  }
+  const cuuint64_t dims[2] = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
+  const cuuint64_t strides[1] = {static_cast<cuuint64_t>(cols) * 2};
+  const cuuint32_t box[2] = {static_cast<cuuint32_t>(box_cols), static_cast<cuuint32_t>(box_rows)};
+  const cuuint32_t estr[2] = {1u, 1u};
+  const CUtensorMapSwizzle swz = box_cols == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
+  const EncodeTiledFn enc = reinterpret_cast<EncodeTiledFn>(fn);
+  const CUresult rc = enc(map, dtype, 2, const_cast<void*>(base), dims, strides, box, estr,
+                          CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return rc == CUDA_SUCCESS ? DGCN_OK : DGCN_ERR_CUDA;
 }
 
 static std::atomic<int> g_cert_on{0};

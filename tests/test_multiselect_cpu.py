@@ -1,5 +1,5 @@
 """CPU restatement of the slab path's multi-select (select_rows_fast_kernel, step 3 in
-deep_gcns_torch_b200/csrc/knn.cuh): histogram the keys below the bound into 256 distance bins, find the
+deep_gcns_torch_b200/csrc/knn.cu): histogram the keys below the bound into 256 distance bins, find the
 bins holding the wanted ranks, sort only those bins' keys, read rank r at position r - (#keys in unmarked
 bins below its bin).  The algorithm - not the CUDA code - is checked here against a full sort."""
 import numpy as np

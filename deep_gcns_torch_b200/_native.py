@@ -54,6 +54,8 @@ _ROW_DTYPE = {torch.float32: DTYPE_F32, torch.bfloat16: DTYPE_BF16, torch.float1
 HALF_ROWS_MAX_C = 1024     # half rows: the forward's widest channel block; the backward's is ...
 HALF_ROWS_MAX_C_BWD = 512  # ... the fp32 backward's own limit
 
+GIN_SAGE = {"gin": 0, "sage": 1, "rsage": 2}   # dgcn_gin_sage
+
 HUB_MIN_DEGREE = 1024      # rows at least this long are aggregated by CTAs instead of one warp
 HUB_SEG_EDGES = 4096       # ... one CTA per segment of this many edges
 
@@ -178,6 +180,10 @@ def _declare(lib):
     lib.dgcn_genconv_aggregate_backward.argtypes = [c_i32, vp, vp, c_i64, c_i64, c_i64, vp, vp, vp, vp,
                                                     ctypes.POINTER(GenconvParamsC), c_i32, vp, vp, c_i32,
                                                     ctypes.POINTER(KeepMaskC), vp, vp, vp, vp, vp, vp]
+    lib.dgcn_gin_sage_aggregate.restype = ctypes.c_int
+    lib.dgcn_gin_sage_aggregate.argtypes = [c_i32, vp, c_i64, c_i64, vp, vp, ctypes.POINTER(CsrHubsC), vp, vp, vp]
+    lib.dgcn_gin_sage_aggregate_backward.restype = ctypes.c_int
+    lib.dgcn_gin_sage_aggregate_backward.argtypes = [c_i32, c_i64, c_i64, vp, vp, vp, vp, vp, vp]
     lib.dgcn_debug_kernel_timing.restype = ctypes.c_int
     lib.dgcn_debug_kernel_timing.argtypes = [c_i32]
     lib.dgcn_debug_kernel_timing_read.restype = ctypes.c_int
@@ -687,6 +693,54 @@ def genconv_aggregate_backward(x_src, x_dst, csr, prm, grad_out, edge_attr=None,
                                                    _ptr(gsrc), _ptr(gdst), _ptr(gea), _ptr(gsc), _stream(dev))
         _check(rc, "dgcn_genconv_aggregate_backward")
     return gsrc, gdst, gea, gsc
+
+
+def _gin_sage_args(rule, x, csr, eps):
+    if rule not in GIN_SAGE:
+        raise ValueError("gin_sage_aggregate: rule must be one of %s, got %r" % (sorted(GIN_SAGE), rule))
+    rowptr, src = csr[0], csr[1]
+    _require_cuda(x, rowptr, src, eps)
+    if x.dim() != 2 or x.dtype != torch.float32:
+        raise RuntimeError("the GIN / SAGE aggregation takes fp32 (N, C) node features, got %s %s"
+                           % (x.dtype, tuple(x.shape)))
+    if rowptr.numel() - 1 != x.shape[0]:
+        raise RuntimeError("gin_sage_aggregate: the CSR graph has %d rows, x has %d" % (rowptr.numel() - 1, x.shape[0]))
+    return rowptr, src, None if (eps is None or rule != "gin") else _f32(eps).reshape(1)
+
+
+def gin_sage_aggregate(rule, x, csr, eps=None):
+    """dgcn_gin_sage_aggregate: (N, C) = sum_j x_j + (1 + eps) x_i ('gin', eps a (1,) tensor or None for 0), or the
+    mean over {j -> i, j != i} + {i} of x_j ('sage') / of x_j - x_i ('rsage'), over the CSR graph (csr_of)."""
+    rowptr, src, eps = _gin_sage_args(rule, x, csr, eps)
+    x = x.detach().contiguous()
+    N, C = x.shape
+    dev = x.device
+    with torch.cuda.device(dev):
+        hubs = None
+        if len(csr) > 3 and csr[3] is not None:
+            items, hrows, counts, n_items = csr[3]
+            partial = torch.empty(n_items * 3 * C, dtype=torch.float32, device=dev)
+            hubs = CsrHubsC(_ptr(items), _ptr(hrows), _ptr(counts), HUB_MIN_DEGREE, HUB_SEG_EDGES, _ptr(partial))
+        out = torch.empty((N, C), dtype=torch.float32, device=dev)
+        rc = lib().dgcn_gin_sage_aggregate(GIN_SAGE[rule], _ptr(x), N, C, _ptr(rowptr), _ptr(src),
+                                           ctypes.byref(hubs) if hubs is not None else None, _ptr(eps), _ptr(out),
+                                           _stream(dev))
+        _check(rc, "dgcn_gin_sage_aggregate")
+    return out
+
+
+def gin_sage_aggregate_backward(rule, grad_out, csr, eps=None):
+    """dgcn_gin_sage_aggregate_backward: grad_x (N, C) fp32 of gin_sage_aggregate for the upstream grad_out."""
+    rowptr, src, eps = _gin_sage_args(rule, grad_out, csr, eps)
+    go = _f32(grad_out)
+    N, C = go.shape
+    dev = go.device
+    with torch.cuda.device(dev):
+        gx = torch.zeros((N, C), dtype=torch.float32, device=dev)
+        rc = lib().dgcn_gin_sage_aggregate_backward(GIN_SAGE[rule], N, C, _ptr(rowptr), _ptr(src), _ptr(eps), _ptr(go),
+                                                    _ptr(gx), _stream(dev))
+        _check(rc, "dgcn_gin_sage_aggregate_backward")
+    return gx
 
 
 def keep_bits(keep):

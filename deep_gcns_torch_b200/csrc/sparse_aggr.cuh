@@ -31,6 +31,8 @@ struct AggrArgs {
   const int32_t* row_list; int n_rows; int run_hubs;
   // dropout folded into the pre-activation (dgcn_keep_mask; KEEP instantiations only)
   const int32_t* keep_bits; int keep_words; float keep_scale;
+  // GIN / GraphSAGE rules (dgcn_gin_sage_aggregate; RULE instantiations only)
+  const float* gin_eps; int relative;
 };
 
 
@@ -106,9 +108,20 @@ __device__ __forceinline__ int chan_of(int lane, int blk, int j) { return blk * 
 // KEEP (with PRE, fp32 rows, no edge features): dropout too - each lane loads its VEC channels' keep bits from the
 // row's words next to the row itself and reads the row as pre_keep(...).
 // (two CTAs per SM for KEEP: the bits' registers would not fit the 85 of three without spilling at NBLK = 2, 4)
-template <typename T, int VEC, int NBLK, int AGGR, int MODE, bool PRE, bool KEEP = false>
+// RULE (dgcn_gin_sage_aggregate: fp32 raw rows, AGGR = ADD, nothing fused): what the row's own x_i adds.
+//   RULE_GIN:       out_i = sum_{j->i} x_j + (1 + eps) x_i, the sum first, then one rounding for the product and
+//                   one for the add (torch_geometric's GINConv in fp32).
+//   RULE_SELF_LOOP: torch_geometric's remove_self_loops + add_self_loops folded into the walk: edges with
+//                   src == i are skipped and counted (a ballot per 32-edge chunk; the count rides in the S state
+//                   through the hub segments' merge, exact below 2^24 self loops per row), c_i = deg - #loops + 1,
+//                   out_i = (sum_{j->i, j!=i} x_j + x_i) / c_i, or with g.relative (x_j - x_i messages, the added
+//                   loop's message is 0) out_i = (sum_{j->i, j!=i} x_j - (c_i - 1) x_i) / c_i.
+constexpr int RULE_NONE = 0, RULE_GIN = 1, RULE_SELF_LOOP = 2;
+template <typename T, int VEC, int NBLK, int AGGR, int MODE, bool PRE, bool KEEP = false, int RULE = RULE_NONE>
 __global__ void __launch_bounds__(256, KEEP ? 2 : (PRE ? 3 : 1)) genconv_aggregate_kernel(const AggrArgs g) {
   static_assert(!KEEP || (PRE && VEC == 4), "keep bits ride on the float4 pre-activation kernels");
+  static_assert(RULE == RULE_NONE || (AGGR == DGCN_AGGR_ADD && !PRE), "the GIN / SAGE rules sum raw rows");
+  constexpr bool kLoop = RULE == RULE_SELF_LOOP;
   constexpr bool HUB = MODE == 1;
   __shared__ float hub_red[HUB ? 8 : 1][3][VEC][32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -140,6 +153,7 @@ __global__ void __launch_bounds__(256, KEEP ? 2 : (PRE ? 3 : 1)) genconv_aggrega
   constexpr bool kPower = (AGGR == DGCN_AGGR_POWER || AGGR == DGCN_AGGR_POWER_SUM);
 
   float m[NBLK][VEC];
+  int n_loops = 0;   // RULE_SELF_LOOP: self loops of the row
 #pragma unroll
   for (int blk = 0; blk < NBLK; ++blk) {
     const int cbase = chan_of<VEC>(lane, blk, 0);
@@ -153,6 +167,7 @@ __global__ void __launch_bounds__(256, KEEP ? 2 : (PRE ? 3 : 1)) genconv_aggrega
       S[j] = 0.f;
       W[j] = (AGGR == DGCN_AGGR_MAX) ? -INFINITY : 0.f;
     }
+    int blk_loops = 0;
     if (blk * 32 * VEC < C) {   // warp-uniform: this channel block exists
       for (int e0 = e_first; e0 < end; e0 += e_step) {
         const int cnt = min(32, end - e0);
@@ -161,6 +176,7 @@ __global__ void __launch_bounds__(256, KEEP ? 2 : (PRE ? 3 : 1)) genconv_aggrega
           my_src = __ldg(g.src + e0 + lane);
           if (g.edge_attr) my_eid = __ldg(g.eid + e0 + lane);
         }
+        if constexpr (kLoop) blk_loops += __popc(__ballot_sync(0xffffffffu, lane < cnt && my_src == row));
         for (int u0 = 0; u0 < cnt; u0 += 4) {
           VecF<VEC> xv[4], ev[4];
           bool have[4];
@@ -170,7 +186,7 @@ __global__ void __launch_bounds__(256, KEEP ? 2 : (PRE ? 3 : 1)) genconv_aggrega
             const int s = __shfl_sync(0xffffffffu, my_src, (u0 + u) & 31);
             int ei = 0;
             if (g.edge_attr) ei = __shfl_sync(0xffffffffu, my_eid, (u0 + u) & 31);   // warp-uniform branch
-            have[u] = live && u0 + u < cnt;
+            have[u] = live && u0 + u < cnt && !(kLoop && s == row);
 #pragma unroll
             for (int j = 0; j < VEC; ++j) {
               xv[u].v[j] = 0.f;
@@ -231,6 +247,10 @@ __global__ void __launch_bounds__(256, KEEP ? 2 : (PRE ? 3 : 1)) genconv_aggrega
         }
       }
     }
+    if constexpr (kLoop) {
+#pragma unroll
+      for (int j = 0; j < VEC; ++j) S[j] = static_cast<float>(blk_loops);   // merged by the hub kernels below
+    }
     if (MODE == 1) {   // merge the 8 warps' states (warp order fixed -> deterministic), publish the segment state
 #pragma unroll
       for (int j = 0; j < VEC; ++j) {
@@ -256,6 +276,7 @@ __global__ void __launch_bounds__(256, KEEP ? 2 : (PRE ? 3 : 1)) genconv_aggrega
               Ws = fmaxf(Ws, Ww);
             } else {
               Ws += Ww;
+              if constexpr (kLoop) Ss += Sw;
             }
           }
           part[cbase + j] = Mx;
@@ -283,6 +304,7 @@ __global__ void __launch_bounds__(256, KEEP ? 2 : (PRE ? 3 : 1)) genconv_aggrega
             Ws = fmaxf(Ws, Ww);
           } else {
             Ws += Ww;
+            if constexpr (kLoop) Ss += Sw;
           }
         }
         M[j] = Mx;
@@ -308,6 +330,7 @@ __global__ void __launch_bounds__(256, KEEP ? 2 : (PRE ? 3 : 1)) genconv_aggrega
       }
       m[blk][j] = live ? r : 0.f;
     }
+    if constexpr (kLoop) if (blk == 0) n_loops = static_cast<int>(S[0]);
   }
   if (AGGR == DGCN_AGGR_SOFTMAX_SUM || AGGR == DGCN_AGGR_POWER_SUM) {   // torch_message.py:60-63,77-80
     const float y = g.y_dev ? __ldg(g.y_dev) : g.y;
@@ -322,7 +345,7 @@ __global__ void __launch_bounds__(256, KEEP ? 2 : (PRE ? 3 : 1)) genconv_aggrega
   // MsgNorm (torch_message.py:95-99) + residual (torch_vertex.py:73)
   float xr[NBLK][VEC];
   float n2m = 0.f, n2x = 0.f;
-  const bool need_x = g.msg_norm || g.add_residual;
+  const bool need_x = RULE != RULE_NONE || g.msg_norm || g.add_residual;
 #pragma unroll
   for (int blk = 0; blk < NBLK; ++blk) {
     const int cbase = chan_of<VEC>(lane, blk, 0);
@@ -369,7 +392,17 @@ __global__ void __launch_bounds__(256, KEEP ? 2 : (PRE ? 3 : 1)) genconv_aggrega
     if (cbase < C) {
       float o[VEC];
 #pragma unroll
-      for (int j = 0; j < VEC; ++j) o[j] = g.add_residual ? fmaf(m[blk][j], f, xr[blk][j]) : m[blk][j] * f;
+      for (int j = 0; j < VEC; ++j) {
+        if (RULE == RULE_GIN) {
+          const float s = __fadd_rn(1.f, g.gin_eps ? __ldg(g.gin_eps) : 0.f);
+          o[j] = __fadd_rn(m[blk][j], __fmul_rn(s, xr[blk][j]));
+        } else if (RULE == RULE_SELF_LOOP) {
+          const float c = static_cast<float>(deg - n_loops + 1);
+          o[j] = __fdiv_rn(g.relative ? fmaf(-(c - 1.f), xr[blk][j], m[blk][j]) : __fadd_rn(m[blk][j], xr[blk][j]), c);
+        } else {
+          o[j] = g.add_residual ? fmaf(m[blk][j], f, xr[blk][j]) : m[blk][j] * f;
+        }
+      }
       float* dst = g.out + static_cast<int64_t>(row) * C + cbase;
       if (VEC == 4) {
         *reinterpret_cast<float4*>(dst) = make_float4(o[0], o[1 % VEC], o[2 % VEC], o[3 % VEC]);

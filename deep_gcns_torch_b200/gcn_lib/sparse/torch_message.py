@@ -88,6 +88,22 @@ class _AggregateFn(torch.autograd.Function):
         return _backward.genconv_aggregate_backward(ctx, grad_out)
 
 
+class _GinSageFn(torch.autograd.Function):
+    """GIN's sum_j x_j + (1 + eps) x_i, or GraphSAGE's mean over {j -> i, j != i} + {i} of x_j ('sage') / x_j - x_i
+    ('rsage'), over the cached CSR graph; see dgcn_gin_sage_aggregate.  eps: GIN's (1,) buffer (no gradient) or None."""
+
+    @staticmethod
+    def forward(ctx, rule, csr, x, eps):
+        ctx.rule, ctx.csr, ctx.eps = rule, csr, eps
+        return _native.gin_sage_aggregate(rule, x, csr, eps)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        gx = _native.gin_sage_aggregate_backward(ctx.rule, grad_out, ctx.csr, ctx.eps) if ctx.needs_input_grad[2] \
+            else None
+        return None, None, gx, None
+
+
 class GenMessagePassing(nn.Module):
     """torch_message.py:8-85."""
 

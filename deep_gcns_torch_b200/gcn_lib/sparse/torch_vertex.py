@@ -1,16 +1,19 @@
 """GENConv and the sparse-layout graph convolutions / blocks - API of the reference's
-gcn_lib/sparse/torch_vertex.py (GENConv :12-88; MRConv :91-103; EdgConv :106-114; GraphConv :239-266; DynConv :267-281;
-blocks :284-352)."""
+gcn_lib/sparse/torch_vertex.py (GENConv :12-88; MRConv :91-103; EdgConv :106-114; SAGEConv / RSAGEConv :136-205;
+GinConv :224-233; GraphConv :239-266; DynConv :267-281; blocks :284-352)."""
+import math
+
 import torch
+import torch.nn.functional as F
 from torch import nn
 
 from ... import _native
 from .._basic_conv import BasicConvLowering, update_running_stats
 from .torch_nn import MLP, BondEncoder
 from .torch_edge import DilatedKnnGraph
-from .torch_message import GenMessagePassing, MsgNorm, _AggregateFn, csr_of
+from .torch_message import GenMessagePassing, MsgNorm, _AggregateFn, _GinSageFn, csr_of
 
-__all__ = ["GENConv", "MRConv", "EdgConv", "GraphConv", "DynConv", "PlainDynBlock", "ResDynBlock", "DenseDynBlock",
+__all__ = ["GENConv", "MRConv", "EdgConv", "GinConv", "SAGEConv", "RSAGEConv", "GraphConv", "DynConv", "PlainDynBlock", "ResDynBlock", "DenseDynBlock",
            "ResGraphBlock", "DenseGraphBlock"]
 
 
@@ -164,10 +167,102 @@ class EdgConv(BasicConvLowering, nn.Module):
                                  None if bn is None else bn.weight, None if bn is None else bn.bias)
 
 
+def _fp32_cuda_input(layer, x, edge_index):
+    _native._require_cuda(x, edge_index)
+    if x.dtype != torch.float32:
+        raise RuntimeError("%s computes in fp32, got %s features" % (layer, x.dtype))
+
+
+class GinConv(nn.Module):
+    """GIN, sparse layout (torch_vertex.py:224-233): torch_geometric's GINConv(MLP([C_in, C_out], act, norm, bias))
+    with eps = 0, not trained (the buffer `eps`, shape [1]):
+        out = nn(agg + (1 + eps) * x),   agg_i = sum over every edge (j -> i) of edge_index of x_j,
+    self loops and duplicate edges counted as given, agg = 0 on a row without in-edges.  In fp32 the order is
+    torch_geometric's: the sum first, then + (1 + eps) * x (one rounding for the product, one for the add).  The
+    aggregation is one pass of the CSR kernel over the cached graph (dgcn_gin_sage_aggregate, forward and backward);
+    the MLP stays torch, so a BatchNorm in it may be an nn.SyncBatchNorm.  `aggr` is accepted and unused, as in the
+    reference.  fp32 CUDA tensors only."""
+
+    def __init__(self, in_channels, out_channels, act="relu", norm=None, bias=True, aggr="add"):
+        super().__init__()
+        self.initial_eps = 0.0
+        self.register_buffer("eps", torch.Tensor([self.initial_eps]))
+        self.nn = MLP([in_channels, out_channels], act, norm, bias)
+
+    def forward(self, x, edge_index):
+        _fp32_cuda_input("GinConv", x, edge_index)
+        csr = csr_of(edge_index, x.size(0))
+        return self.nn(_GinSageFn.apply("gin", csr, x, self.eps))
+
+
+class SAGEConv(nn.Module):
+    """GraphSAGE, sparse layout: the reference's SAGEConv (torch_vertex.py:136-189) on torch_geometric's older
+    SAGEConv(C_in, C_out, normalize, bias) layout - `weight` (C_in, C_out), `bias` (C_out) when `bias`, both uniform
+    in +-1/sqrt(C_in); normalize = norm is not None - with the reference's message and update:
+        forward(x, edge_index, size=None): every self loop removed and one added per node (skipped when `size` is
+          given, as in the reference), so row i's set is {j : (j -> i), j != i} + {i}, c_i = its size;
+        message x_j W, or (x_j - x_i) W when `relative` (the added self loop's message is 0); mean over the set;
+        out = nn(cat[x, aggr]) (+ bias), then F.normalize(out, p=2, dim=-1) when normalize.
+    The message is linear, so the mean runs on the raw rows in the CSR kernel over the cached graph
+    (dgcn_gin_sage_aggregate: (sum_{j != i} x_j + x_i) / c_i, relative (sum_{j != i} x_j - (c_i - 1) x_i) / c_i,
+    equal to the reference up to re-association) and W, nn, bias and the normalisation stay torch.  With `size`,
+    the mean over edge_index as given (an empty row gives 0).  fp32 CUDA tensors only."""
+
+    def __init__(self, in_channels, out_channels, nn, norm=True, bias=True, relative=False, **kwargs):
+        super().__init__()
+        self.in_channels, self.out_channels = in_channels, out_channels
+        self.relative = relative
+        self.normalize = norm is not None
+        self.weight = torch.nn.Parameter(torch.Tensor(in_channels, out_channels))
+        if bias:
+            self.bias = torch.nn.Parameter(torch.Tensor(out_channels))
+        else:
+            self.register_parameter("bias", None)
+        self.reset_parameters()
+        self.nn = nn
+
+    def reset_parameters(self):
+        bound = 1.0 / math.sqrt(self.in_channels)
+        for p in (self.weight, self.bias):
+            if p is not None:
+                p.data.uniform_(-bound, bound)
+
+    def forward(self, x, edge_index, size=None):
+        x = x.unsqueeze(-1) if x.dim() == 1 else x
+        _fp32_cuda_input(type(self).__name__, x, edge_index)
+        if size is None:
+            csr = csr_of(edge_index, x.size(0))
+            aggr = _GinSageFn.apply("rsage" if self.relative else "sage", csr, x, None)
+        else:
+            if tuple(size) != (x.size(0), x.size(0)):
+                raise NotImplementedError("SAGEConv: size must be None or (N, N) with N = x.size(0), got %s"
+                                          % (tuple(size),))
+            aggr, csr = _aggregate_rows("mean", x, edge_index)
+            if self.relative:
+                deg = (csr[0][1:] - csr[0][:-1]).unsqueeze(1)
+                aggr = torch.where(deg > 0, aggr - x, torch.zeros_like(aggr))
+        out = self.nn(torch.cat((x, torch.matmul(aggr, self.weight)), dim=1))
+        if self.bias is not None:
+            out = out + self.bias
+        if self.normalize:
+            out = F.normalize(out, p=2, dim=-1)
+        return out
+
+
+class RSAGEConv(SAGEConv):
+    """torch_vertex.py:192-205: SAGEConv with nn = MLP([C_out + C_in, C_out], act, norm, bias)."""
+
+    def __init__(self, in_channels, out_channels, act="relu", norm=None, bias=True, relative=False):
+        nn_ = MLP([out_channels + in_channels, out_channels], act, norm, bias)
+        super().__init__(in_channels, out_channels, nn_, norm, bias, relative)
+
+
 class GraphConv(nn.Module):
-    """Static graph convolution, sparse layout (torch_vertex.py:239-266).  'edge' (EdgConv) and 'mr' (MRConv) run on
-    the CSR kernels; the other variants are thin wrappers over third-party PyG convolutions in the reference
-    (GATConv, GCNConv, GINConv, SAGEConv) and are not part of the rebuilt path."""
+    """Static graph convolution, sparse layout (torch_vertex.py:239-266).  'edge' (EdgConv), 'mr' (MRConv), 'gin'
+    (GinConv), 'sage' and 'rsage' (RSAGEConv, relative False / True) run on the CSR kernels.  'gat' and 'gcn' wrap
+    torch_geometric's GATConv / GCNConv in the reference, whose attention, normalisation and state_dict layout changed
+    across the torch_geometric versions its install can pick; they are not part of the rebuilt path.  `heads` is
+    accepted and unused."""
 
     def __init__(self, in_channels, out_channels, conv="edge", act="relu", norm=None, bias=True, heads=8):
         super().__init__()
@@ -175,9 +270,15 @@ class GraphConv(nn.Module):
             self.gconv = EdgConv(in_channels, out_channels, act, norm, bias)
         elif conv.lower() == "mr":
             self.gconv = MRConv(in_channels, out_channels, act, norm, bias)
-        elif conv.lower() in ("gat", "gcn", "gin", "sage", "rsage"):
+        elif conv.lower() == "gin":
+            self.gconv = GinConv(in_channels, out_channels, act, norm, bias)
+        elif conv.lower() == "sage":
+            self.gconv = RSAGEConv(in_channels, out_channels, act, norm, bias, False)
+        elif conv.lower() == "rsage":
+            self.gconv = RSAGEConv(in_channels, out_channels, act, norm, bias, True)
+        elif conv.lower() in ("gat", "gcn"):
             raise NotImplementedError("conv {}: a torch_geometric layer in the reference; the sparse-layout path here "
-                                      "covers 'edge' and 'mr'".format(conv))
+                                      "covers 'edge', 'mr', 'gin', 'sage' and 'rsage'".format(conv))
         else:
             raise NotImplementedError("conv {} is not implemented".format(conv))
 

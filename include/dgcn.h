@@ -377,6 +377,31 @@ int dgcn_res_plus_backward_gy(const float* h, int64_t N, int64_t C, const float*
 int dgcn_res_plus_backward_dh(const float* g_y, const float* h, int64_t N, int64_t C, const float* a, const float* b,
                               const float* d, const float* grad_skip, float* grad_h, dgcn_stream_t stream);
 
+/* GIN and GraphSAGE aggregation in the sparse layout (the message passing of gcn_lib/sparse/torch_vertex.py:224-233,
+ * torch_geometric's GINConv with eps not trained, and :136-205, the SAGEConv subclass; the MLP, the weight GEMM, the
+ * bias and the normalisation stay with the caller).  Over dgcn_csr_build's rowptr (N+1) / src (E) of edge_index:
+ *   DGCN_GIN:   out_i = sum_{j->i} x_j + (1 + eps) * x_i  over every edge as given (self loops and duplicates
+ *               included, an empty row sums to 0); the sum first, then + fl(fl(1 + eps) * x_i) - the fp32 order of
+ *               torch_geometric's GINConv.  eps: (1) DEVICE scalar (the layer's buffer) or NULL for 0.
+ *   DGCN_SAGE:  torch_geometric's remove_self_loops + add_self_loops, folded into the walk: with c_i = (number of
+ *               edges j -> i with j != i) + 1, out_i = (sum_{j->i, j != i} x_j + x_i) / c_i;
+ *   DGCN_RSAGE: the same set with messages x_j - x_i (the added loop's message is 0):
+ *               out_i = (sum_{j->i, j != i} x_j - (c_i - 1) * x_i) / c_i.
+ * x (N, C) fp32 row-major, out (N, C) fp32.  C <= 1024 when C % 4 == 0 and x, out are 16-byte aligned, else
+ * C <= 256; anything else returns DGCN_ERR_UNSUPPORTED.  hubs: dgcn_csr_hubs or NULL (rows of in-degree >=
+ * min_degree are then aggregated in segments, with the same result up to fp32 re-association). */
+enum dgcn_gin_sage { DGCN_GIN = 0, DGCN_SAGE = 1, DGCN_RSAGE = 2 };
+int dgcn_gin_sage_aggregate(int32_t rule, const float* x, int64_t N, int64_t C, const int32_t* rowptr,
+                            const int32_t* src, const dgcn_csr_hubs* hubs /* may be NULL */, const float* eps,
+                            float* out, dgcn_stream_t stream);
+/* Gradient of dgcn_gin_sage_aggregate w.r.t. x: grad_x (N, C) must be zero-initialised by the caller (rows are
+ * accumulated with atomics, so the order of the additions - and the last bits - varies from run to run).  Every
+ * source of an edge j -> i receives grad_out_i (GIN) or grad_out_i / c_i (SAGE, RSAGE; edges with j != i only); row i
+ * receives (1 + eps) * grad_out_i (GIN), grad_out_i / c_i (SAGE) or -(c_i - 1) / c_i * grad_out_i (RSAGE).
+ * C <= 1024. */
+int dgcn_gin_sage_aggregate_backward(int32_t rule, int64_t N, int64_t C, const int32_t* rowptr, const int32_t* src,
+                                     const float* eps, const float* grad_out, float* grad_x, dgcn_stream_t stream);
+
 /* EdgeConv in the sparse layout.
  * Replaces gcn_lib/sparse/torch_vertex.py:106-114 (EdgConv = torch_geometric's EdgeConv with aggr 'max' around
  * MLP([2*C_in, C_out], act, norm, bias), gcn_lib/sparse/torch_nn.py:50-68).  The order is Linear -> norm -> act

@@ -235,7 +235,8 @@ def _check(rc, what):
         l = lib()
         msg = l.dgcn_status_string(rc).decode()
         extra = l.dgcn_last_cuda_error().decode() if rc == -4 else ""
-        raise RuntimeError("%s failed: %s %s" % (what, msg, extra))
+        # DGCN_ERR_UNSUPPORTED: a valid request the kernels do not cover (NotImplementedError is a RuntimeError)
+        raise (NotImplementedError if rc == -2 else RuntimeError)("%s failed: %s %s" % (what, msg, extra))
 
 
 def _ptr(t):

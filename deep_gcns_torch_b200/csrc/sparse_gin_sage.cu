@@ -32,6 +32,8 @@ static int dispatch_gin_sage(const AggrArgs& g, bool vec4, cudaStream_t s) {
     else if (C <= 64) launch_gin_sage<1, 2, RULE>(g, s);
     else if (C <= 128) launch_gin_sage<1, 4, RULE>(g, s);
     else if (C <= 256) launch_gin_sage<1, 8, RULE>(g, s);
+    else if (C <= 512) launch_gin_sage<1, 16, RULE>(g, s);
+    else if (C <= 1024) launch_gin_sage<1, 32, RULE>(g, s);
     else return DGCN_ERR_UNSUPPORTED;
   }
   DGCN_LAUNCH_CHECK();

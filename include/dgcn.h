@@ -387,9 +387,10 @@ int dgcn_res_plus_backward_dh(const float* g_y, const float* h, int64_t N, int64
  *               edges j -> i with j != i) + 1, out_i = (sum_{j->i, j != i} x_j + x_i) / c_i;
  *   DGCN_RSAGE: the same set with messages x_j - x_i (the added loop's message is 0):
  *               out_i = (sum_{j->i, j != i} x_j - (c_i - 1) * x_i) / c_i.
- * x (N, C) fp32 row-major, out (N, C) fp32.  C <= 1024 when C % 4 == 0 and x, out are 16-byte aligned, else
- * C <= 256; anything else returns DGCN_ERR_UNSUPPORTED.  hubs: dgcn_csr_hubs or NULL (rows of in-degree >=
- * min_degree are then aggregated in segments, with the same result up to fp32 re-association). */
+ * x (N, C) fp32 row-major, out (N, C) fp32, C <= 1024 (float4 lanes when C % 4 == 0 and x, out are 16-byte
+ * aligned, one channel per lane otherwise, with the same result); C > 1024 returns DGCN_ERR_UNSUPPORTED.  hubs:
+ * dgcn_csr_hubs or NULL (rows of in-degree >= min_degree are then aggregated in segments, with the same result up to
+ * fp32 re-association). */
 enum dgcn_gin_sage { DGCN_GIN = 0, DGCN_SAGE = 1, DGCN_RSAGE = 2 };
 int dgcn_gin_sage_aggregate(int32_t rule, const float* x, int64_t N, int64_t C, const int32_t* rowptr,
                             const int32_t* src, const dgcn_csr_hubs* hubs /* may be NULL */, const float* eps,

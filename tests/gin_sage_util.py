@@ -10,6 +10,10 @@
 - gin_aggr / sage_aggr: the aggregations restated functionally on any device and dtype (the fp64 references of the
   GPU tests): remove_self_loops + add_self_loops + mean for SAGE, exactly as torch_geometric composes them.
 - exact_graph / exact_features: the exact-arithmetic fixtures of tests/test_gin_sage_gpu.py.
+- gin_aggr_chunked / sage_aggr_chunked / gin_sage_grad_chunked: the same aggregations and their gradient written out,
+  in fp64 over a whole ogbn-sized graph a chunk of edges at a time (tests/test_gin_sage_scale_gpu.py).
+- loop_positions / plant_self_loops / exact_magnitudes: the self loops that test file plants at the hub kernels'
+  segment and ballot boundaries, and the bounds that keep its integer fixtures exact in fp32.
 """
 import sys
 
@@ -116,6 +120,138 @@ def exact_graph(N, g, hub=0):
 def exact_features(N, C, g):
     """(N, C) fp32 integers in [-4, 4]."""
     return torch.randint(-4, 5, (N, C), generator=g).float()
+
+
+# ---- whole-graph fp64 references, a chunk of edges at a time --------------------------------------------------------
+# At the ogbn shapes one gather of every edge's row would take tens of GiB; the chunked forms keep one chunk's gathered
+# rows (in the reference's dtype) below REF_CHUNK_BYTES and sum with index_add_ into one (N, C) accumulator.
+REF_CHUNK_BYTES = 2**30
+
+
+def edge_chunks(edge_index, width, device, drop_self=False, itemsize=8):
+    """(src, dst) int64 on `device` for consecutive chunks of edge_index's edges, each chunk small enough that its
+    gathered (chunk, width) rows of `itemsize`-byte values stay below REF_CHUNK_BYTES; drop_self: without the self
+    loops."""
+    step = max(1, REF_CHUNK_BYTES // (itemsize * max(width, 1)))
+    for e0 in range(0, edge_index.shape[1], step):
+        src, dst = (t.long().to(device) for t in edge_index[:, e0:e0 + step])
+        if drop_self:
+            keep = src != dst
+            src, dst = src[keep], dst[keep]
+        yield src, dst
+
+
+def sage_counts(edge_index, N, device=None, dtype=torch.float64):
+    """c_i = (number of edges j -> i with j != i) + 1: the size of row i's set after remove_self_loops +
+    add_self_loops, counted on edge_index (not on any CSR)."""
+    device = edge_index.device if device is None else device
+    c = torch.ones(N, dtype=dtype, device=device)
+    for _src, dst in edge_chunks(edge_index, 1, device, drop_self=True):
+        c.index_add_(0, dst, torch.ones_like(dst, dtype=dtype))
+    return c
+
+
+def gin_aggr_chunked(x, edge_index, eps=0.0, dtype=torch.float64):
+    """gin_aggr in `dtype` (x in any dtype: rows are converted as they are gathered)."""
+    agg = torch.zeros(x.shape, dtype=dtype, device=x.device)
+    for src, dst in edge_chunks(edge_index, x.shape[1], x.device):
+        agg.index_add_(0, dst, x.index_select(0, src).to(dtype))
+    return agg.add_(x.to(dtype), alpha=1 + eps)
+
+
+def sage_aggr_chunked(x, edge_index, relative=False, dtype=torch.float64):
+    """sage_aggr in `dtype`: s_i = sum over the edges j -> i, j != i of x_j, then (s_i + x_i) / c_i, or with
+    relative (s_i - (c_i - 1) x_i) / c_i - the sum of the messages x_j - x_i over the same set, where the added self
+    loop's message is 0."""
+    s = torch.zeros(x.shape, dtype=dtype, device=x.device)
+    for src, dst in edge_chunks(edge_index, x.shape[1], x.device, drop_self=True):
+        s.index_add_(0, dst, x.index_select(0, src).to(dtype))
+    c = sage_counts(edge_index, x.shape[0], x.device, dtype).unsqueeze(1)
+    if relative:
+        s.addcmul_(c - 1, x.to(dtype), value=-1)
+    else:
+        s.add_(x.to(dtype))
+    return s.div_(c)
+
+
+def gin_sage_grad_chunked(rule, grad_out, edge_index, eps=0.0, dtype=torch.float64):
+    """The gradient w.r.t. x of sum(out * grad_out) for out = gin_aggr / sage_aggr, written out: every edge j -> i
+    (j != i for SAGE) sends g_i (GIN) or g_i / c_i (SAGE, RSAGE) to row j, and row i receives (1 + eps) g_i, g_i / c_i
+    or -(c_i - 1) / c_i g_i.  In `dtype`, a chunk of edges at a time."""
+    ge = grad_out.to(dtype, copy=True)
+    if rule == "gin":
+        gx = ge * (1 + eps)
+    else:
+        c = sage_counts(edge_index, ge.shape[0], ge.device, dtype).unsqueeze(1)
+        ge.div_(c)
+        gx = ge.clone() if rule == "sage" else ge * -(c - 1)
+    for src, dst in edge_chunks(edge_index, ge.shape[1], ge.device, drop_self=rule != "gin"):
+        gx.index_add_(0, src, ge.index_select(0, dst))
+    return gx
+
+
+# ---- self loops planted at the hub kernels' boundaries -------------------------------------------------------------
+SEG_EDGES = 4096                      # _native.HUB_SEG_EDGES: edges per hub segment
+BIG_ROW_LOOPS = 475_713               # on the 10^6-edge row: c = 10^6 - 475,713 + 1 = 2^19
+
+
+def loop_positions(deg):
+    """Which of a planted row's edges (0 .. deg - 1, in the row's order) become self loops, by the row's degree:
+    1023 / 1024 all of them (c = 1 on the last one-warp row and on the first hub row); 4096 its first 32 (one full
+    ballot chunk); 4097 its last (the only edge of its second segment); 8192 every other edge of its second segment
+    only; 10^6 BIG_ROW_LOOPS spread evenly over all 245 segments (a count above 2^16 carried through the merge,
+    c = 2^19).  None for any other degree."""
+    if deg in (1023, 1024):
+        return torch.arange(deg)
+    if deg == 4096:
+        return torch.arange(32)
+    if deg == 4097:
+        return torch.tensor([4096])
+    if deg == 8192:
+        return torch.arange(SEG_EDGES, 8192, 2)
+    if deg == 10**6:
+        return torch.arange(BIG_ROW_LOOPS) * deg // BIG_ROW_LOOPS
+    return None
+
+
+def plant_self_loops(edge_index, planted, loop_rows=(), every=97):
+    """Turns edges of edge_index into self loops in place (edge_index[0] = edge_index[1]):
+    - planted ({row: degree}): the edges loop_positions(degree) of the row, counted in edge_index order - the order a
+      stable CSR build keeps within a row - and no other edge of the row (a loop drawn there moves to another source);
+    - loop_rows: every edge of these rows;
+    - of every other row, the edges at the indices of edge_index divisible by `every`.
+    Returns the rows the first two rules fixed (planted rows of another degree take the third)."""
+    plan = {r: loop_positions(int(d)) for r, d in planted.items()}
+    plan = {r: pos for r, pos in plan.items() if pos is not None}
+    plan.update({r: None for r in loop_rows})
+    for r, pos in plan.items():
+        at = (edge_index[1] == r).nonzero().squeeze(1)
+        assert r not in planted or at.numel() == planted[r], (r, at.numel(), planted[r])
+        if pos is not None:
+            drawn = at[edge_index[0, at] == r]
+            edge_index[0, drawn] = r - 1 if r > 0 else 1
+            at = at[pos.to(at.device)]
+        edge_index[0, at] = r
+    idx = torch.arange(0, edge_index.shape[1], every, device=edge_index.device)
+    fixed = torch.tensor(sorted(plan), dtype=edge_index.dtype, device=edge_index.device)
+    idx = idx[~torch.isin(edge_index[1, idx], fixed)]
+    edge_index[0, idx] = edge_index[1, idx]
+    return sorted(plan)
+
+
+def exact_magnitudes(edge_index, N):
+    """Bounds, on integer features in [-4, 4] and upstream gradients g_i = k_i / 4 (GIN) or c_i k_i / 4 (SAGE) with
+    |k_i| <= 4, of every fp32 value the GIN / SAGE kernels form, forward and backward, on this graph: (forward, the
+    largest |partial sum| of a row's messages plus its own term; backward, the largest |sum| one row's gradient
+    collects).  Below 2^22 every such value is a multiple of 1/16 (GIN's fl(1.25 x_i) and fl(1.25 g_i)) or 1/4 held
+    exactly, in any order of the additions."""
+    dev = edge_index.device
+    indeg = torch.bincount(edge_index[1], minlength=N)
+    outdeg = torch.bincount(edge_index[0], minlength=N)
+    c = sage_counts(edge_index, N, dev, torch.float64)
+    fwd = max(float(indeg.max()) * 4 + 5, float(((c - 1) * 4 * 2).max()))       # GIN; RSAGE sum - (c - 1) x_i
+    bwd = float((outdeg.double() + (c - 1).clamp(min=1.25)).max())                # each scatter |k/4| <= 1
+    return fwd, bwd
 
 
 def sixteenths(shape, g):

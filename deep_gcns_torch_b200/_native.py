@@ -181,7 +181,8 @@ def _declare(lib):
                                                     ctypes.POINTER(GenconvParamsC), c_i32, vp, vp, c_i32,
                                                     ctypes.POINTER(KeepMaskC), vp, vp, vp, vp, vp, vp]
     lib.dgcn_gin_sage_aggregate.restype = ctypes.c_int
-    lib.dgcn_gin_sage_aggregate.argtypes = [c_i32, vp, c_i64, c_i64, vp, vp, ctypes.POINTER(CsrHubsC), vp, vp, vp]
+    lib.dgcn_gin_sage_aggregate.argtypes = [c_i32, c_i32, vp, c_i64, c_i64, vp, vp, ctypes.POINTER(CsrHubsC), vp, vp,
+                                            vp]
     lib.dgcn_gin_sage_aggregate_backward.restype = ctypes.c_int
     lib.dgcn_gin_sage_aggregate_backward.argtypes = [c_i32, c_i64, c_i64, vp, vp, vp, vp, vp, vp]
     lib.dgcn_debug_kernel_timing.restype = ctypes.c_int
@@ -294,7 +295,7 @@ def _f32(t):
 
 
 def aggregate_rows(x_src, x_dst=None, edge_attr=None, pre=None, backward=False):
-    """(dgcn_dtype, x_src, x_dst, edge_attr) as the GENConv aggregate kernels read them.
+    """(dgcn_dtype, x_src, x_dst, edge_attr) as the GENConv and GIN / GraphSAGE aggregate kernels read them.
 
     bf16 / fp16 rows are read as they are (widened to fp32 in registers: bit for bit the result of the fp32 copy)
     when x_src is bf16 or fp16, x_dst and edge_attr (where given) have the same dtype, C % 4 == 0,
@@ -696,24 +697,27 @@ def genconv_aggregate_backward(x_src, x_dst, csr, prm, grad_out, edge_attr=None,
     return gsrc, gdst, gea, gsc
 
 
-def _gin_sage_args(rule, x, csr, eps):
+def _gin_sage_args(rule, x, csr, eps, half_rows=False):
+    """half_rows: x may also be bf16 / fp16 (the forward's node features; the backward's gradient is fp32)."""
     if rule not in GIN_SAGE:
         raise ValueError("gin_sage_aggregate: rule must be one of %s, got %r" % (sorted(GIN_SAGE), rule))
     rowptr, src = csr[0], csr[1]
     _require_cuda(x, rowptr, src, eps)
-    if x.dim() != 2 or x.dtype != torch.float32:
-        raise RuntimeError("the GIN / SAGE aggregation takes fp32 (N, C) node features, got %s %s"
-                           % (x.dtype, tuple(x.shape)))
+    if x.dim() != 2 or x.dtype not in (_ROW_DTYPE if half_rows else (torch.float32,)):
+        raise RuntimeError("the GIN / SAGE aggregation takes %s (N, C) node features, got %s %s"
+                           % ("fp32, bf16 or fp16" if half_rows else "fp32", x.dtype, tuple(x.shape)))
     if rowptr.numel() - 1 != x.shape[0]:
         raise RuntimeError("gin_sage_aggregate: the CSR graph has %d rows, x has %d" % (rowptr.numel() - 1, x.shape[0]))
     return rowptr, src, None if (eps is None or rule != "gin") else _f32(eps).reshape(1)
 
 
 def gin_sage_aggregate(rule, x, csr, eps=None):
-    """dgcn_gin_sage_aggregate: (N, C) = sum_j x_j + (1 + eps) x_i ('gin', eps a (1,) tensor or None for 0), or the
-    mean over {j -> i, j != i} + {i} of x_j ('sage') / of x_j - x_i ('rsage'), over the CSR graph (csr_of)."""
-    rowptr, src, eps = _gin_sage_args(rule, x, csr, eps)
-    x = x.detach().contiguous()
+    """dgcn_gin_sage_aggregate: (N, C) fp32 = sum_j x_j + (1 + eps) x_i ('gin', eps a (1,) tensor or None for 0), or
+    the mean over {j -> i, j != i} + {i} of x_j ('sage') / of x_j - x_i ('rsage'), over the CSR graph (csr_of).
+    x fp32, bf16 or fp16: half rows are read as they are where aggregate_rows allows, else as an fp32 copy; either
+    way the result is bit for bit that of the call on x.float()."""
+    rowptr, src, eps = _gin_sage_args(rule, x, csr, eps, half_rows=True)
+    dtype, x, _, _ = aggregate_rows(x)
     N, C = x.shape
     dev = x.device
     with torch.cuda.device(dev):
@@ -723,7 +727,7 @@ def gin_sage_aggregate(rule, x, csr, eps=None):
             partial = torch.empty(n_items * 3 * C, dtype=torch.float32, device=dev)
             hubs = CsrHubsC(_ptr(items), _ptr(hrows), _ptr(counts), HUB_MIN_DEGREE, HUB_SEG_EDGES, _ptr(partial))
         out = torch.empty((N, C), dtype=torch.float32, device=dev)
-        rc = lib().dgcn_gin_sage_aggregate(GIN_SAGE[rule], _ptr(x), N, C, _ptr(rowptr), _ptr(src),
+        rc = lib().dgcn_gin_sage_aggregate(dtype, GIN_SAGE[rule], _ptr(x), N, C, _ptr(rowptr), _ptr(src),
                                            ctypes.byref(hubs) if hubs is not None else None, _ptr(eps), _ptr(out),
                                            _stream(dev))
         _check(rc, "dgcn_gin_sage_aggregate")

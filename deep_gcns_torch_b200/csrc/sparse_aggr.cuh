@@ -1,6 +1,7 @@
 // GENConv aggregate kernel (message + aggregate + MsgNorm + residual over a CSR-by-destination graph), shared by
 // sparse_fwd.cu (fp32 rows) and sparse_fwd_half.cu (bf16 / fp16 rows, their own translation unit so the build
-// compiles both halves in parallel).
+// compiles both halves in parallel), and with its GIN / GraphSAGE rules by sparse_gin_sage.cu and
+// sparse_gin_sage_half.cu.
 //
 // One warp owns one destination row; lanes own channels (VEC consecutive channels per
 // lane per channel block, so a warp reads a source row as one coalesced segment).
@@ -108,7 +109,7 @@ __device__ __forceinline__ int chan_of(int lane, int blk, int j) { return blk * 
 // KEEP (with PRE, fp32 rows, no edge features): dropout too - each lane loads its VEC channels' keep bits from the
 // row's words next to the row itself and reads the row as pre_keep(...).
 // (two CTAs per SM for KEEP: the bits' registers would not fit the 85 of three without spilling at NBLK = 2, 4)
-// RULE (dgcn_gin_sage_aggregate: fp32 raw rows, AGGR = ADD, nothing fused): what the row's own x_i adds.
+// RULE (dgcn_gin_sage_aggregate: raw rows of any T, AGGR = ADD, nothing fused): what the row's own x_i adds.
 //   RULE_GIN:       out_i = sum_{j->i} x_j + (1 + eps) x_i, the sum first, then one rounding for the product and
 //                   one for the add (torch_geometric's GINConv in fp32).
 //   RULE_SELF_LOOP: torch_geometric's remove_self_loops + add_self_loops folded into the walk: edges with
@@ -444,5 +445,34 @@ static int launch_aggr(const AggrArgs& g, cudaStream_t stream) {
 
 // bf16 / fp16 rows (sparse_fwd_half.cu): VEC = 4 and the NBLK the fp32 dispatch picks for C, no pre-activation
 int launch_aggr_half(const AggrArgs& g, int dtype, cudaStream_t stream);
+
+// GIN / GraphSAGE forward (dgcn_gin_sage_aggregate): the RULE kernels on rows of type T, row kernel and hub kernels
+template <typename T, int VEC, int NBLK, int RULE>
+static void launch_gin_sage(const AggrArgs& g, cudaStream_t stream) {
+  const unsigned grid = static_cast<unsigned>(ceil_div(g.n_rows, 8));
+  KernelTimer timer(stream, "gin_sage");
+  if (grid) genconv_aggregate_kernel<T, VEC, NBLK, DGCN_AGGR_ADD, 0, false, false, RULE><<<grid, 256, 0, stream>>>(g);
+  if (g.hub_rows) {
+    genconv_aggregate_kernel<T, VEC, NBLK, DGCN_AGGR_ADD, 1, false, false, RULE><<<4 * device_sm_count(), 256, 0, stream>>>(g);
+    genconv_aggregate_kernel<T, VEC, NBLK, DGCN_AGGR_ADD, 2, false, false, RULE><<<32, 256, 0, stream>>>(g);
+  }
+}
+
+// The VEC 4 GIN / GraphSAGE launch for C channels, on fp32 rows and on half rows alike: one channel block per 128
+// channels, so a half call sums each channel over the same lanes and edges in the same order as the fp32 call.
+template <typename T, int RULE>
+static int launch_gin_sage_vec4(const AggrArgs& g, cudaStream_t s) {
+  const int C = g.C;
+  if (C <= 128) launch_gin_sage<T, 4, 1, RULE>(g, s);
+  else if (C <= 256) launch_gin_sage<T, 4, 2, RULE>(g, s);
+  else if (C <= 512) launch_gin_sage<T, 4, 4, RULE>(g, s);
+  else if (C <= 1024) launch_gin_sage<T, 4, 8, RULE>(g, s);
+  else return DGCN_ERR_UNSUPPORTED;
+  DGCN_LAUNCH_CHECK();
+  return DGCN_OK;
+}
+
+// bf16 / fp16 rows (sparse_gin_sage_half.cu): launch_gin_sage_vec4 on __nv_bfloat16 / __half rows
+int launch_gin_sage_half(const AggrArgs& g, int dtype, bool gin, cudaStream_t stream);
 
 }  // namespace dgcn

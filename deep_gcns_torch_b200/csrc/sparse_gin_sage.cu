@@ -1,41 +1,24 @@
 // Sparse path: the aggregation of GIN and GraphSAGE (gcn_lib/sparse/torch_vertex.py:136-205, 224-233) over the
 // CSR-by-destination graph, forward and backward.  The forward is the GENConv aggregate kernel (sparse_aggr.cuh) on
-// the raw source rows with a RULE for the row's own term: warp per row, float4 lanes, hub segments.  The backward is
-// linear in the upstream gradient: one warp per destination row scatters its scaled gradient row to the sources with
-// atomics, as the raw-message backward of dgcn_genconv_aggregate_backward does, and adds the self term to its own row.
+// the raw source rows with a RULE for the row's own term: warp per row, float4 lanes, hub segments (bf16 / fp16
+// rows: sparse_gin_sage_half.cu).  The backward is linear in the upstream gradient and does not read x: one warp per
+// destination row scatters its scaled gradient row to the sources with atomics, as the raw-message backward of
+// dgcn_genconv_aggregate_backward does, and adds the self term to its own row.
 #include "sparse_aggr.cuh"
 
 namespace dgcn {
 
-template <int VEC, int NBLK, int RULE>
-static void launch_gin_sage(const AggrArgs& g, cudaStream_t stream) {
-  const unsigned grid = static_cast<unsigned>(ceil_div(g.n_rows, 8));
-  KernelTimer timer(stream, "gin_sage");
-  if (grid) genconv_aggregate_kernel<float, VEC, NBLK, DGCN_AGGR_ADD, 0, false, false, RULE><<<grid, 256, 0, stream>>>(g);
-  if (g.hub_rows) {
-    genconv_aggregate_kernel<float, VEC, NBLK, DGCN_AGGR_ADD, 1, false, false, RULE><<<4 * device_sm_count(), 256, 0, stream>>>(g);
-    genconv_aggregate_kernel<float, VEC, NBLK, DGCN_AGGR_ADD, 2, false, false, RULE><<<32, 256, 0, stream>>>(g);
-  }
-}
-
 template <int RULE>
 static int dispatch_gin_sage(const AggrArgs& g, bool vec4, cudaStream_t s) {
+  if (vec4) return launch_gin_sage_vec4<float, RULE>(g, s);
   const int C = g.C;
-  if (vec4) {
-    if (C <= 128) launch_gin_sage<4, 1, RULE>(g, s);
-    else if (C <= 256) launch_gin_sage<4, 2, RULE>(g, s);
-    else if (C <= 512) launch_gin_sage<4, 4, RULE>(g, s);
-    else if (C <= 1024) launch_gin_sage<4, 8, RULE>(g, s);
-    else return DGCN_ERR_UNSUPPORTED;
-  } else {
-    if (C <= 32) launch_gin_sage<1, 1, RULE>(g, s);
-    else if (C <= 64) launch_gin_sage<1, 2, RULE>(g, s);
-    else if (C <= 128) launch_gin_sage<1, 4, RULE>(g, s);
-    else if (C <= 256) launch_gin_sage<1, 8, RULE>(g, s);
-    else if (C <= 512) launch_gin_sage<1, 16, RULE>(g, s);
-    else if (C <= 1024) launch_gin_sage<1, 32, RULE>(g, s);
-    else return DGCN_ERR_UNSUPPORTED;
-  }
+  if (C <= 32) launch_gin_sage<float, 1, 1, RULE>(g, s);
+  else if (C <= 64) launch_gin_sage<float, 1, 2, RULE>(g, s);
+  else if (C <= 128) launch_gin_sage<float, 1, 4, RULE>(g, s);
+  else if (C <= 256) launch_gin_sage<float, 1, 8, RULE>(g, s);
+  else if (C <= 512) launch_gin_sage<float, 1, 16, RULE>(g, s);
+  else if (C <= 1024) launch_gin_sage<float, 1, 32, RULE>(g, s);
+  else return DGCN_ERR_UNSUPPORTED;
   DGCN_LAUNCH_CHECK();
   return DGCN_OK;
 }
@@ -115,15 +98,16 @@ using namespace dgcn;
 
 extern "C" {
 
-int dgcn_gin_sage_aggregate(int32_t rule, const float* x, int64_t N, int64_t C, const int32_t* rowptr,
+int dgcn_gin_sage_aggregate(int32_t dtype, int32_t rule, const void* x, int64_t N, int64_t C, const int32_t* rowptr,
                             const int32_t* src, const dgcn_csr_hubs* hubs, const float* eps, float* out,
                             dgcn_stream_t stream) {
   if (!x || !rowptr || !src || !out || N < 0 || C <= 0) return DGCN_ERR_BAD_ARG;
+  if (dtype != DGCN_F32 && dtype != DGCN_BF16 && dtype != DGCN_F16) return DGCN_ERR_BAD_ARG;
   if (rule != DGCN_GIN && rule != DGCN_SAGE && rule != DGCN_RSAGE) return DGCN_ERR_BAD_ARG;
   if (N == 0) return DGCN_OK;
   if (N > (1ll << 31) - 1) return DGCN_ERR_UNSUPPORTED;
   AggrArgs g{};
-  g.x_src = x; g.x_dst = x; g.N = static_cast<int>(N); g.C = static_cast<int>(C);
+  g.x_src = static_cast<const float*>(x); g.x_dst = g.x_src; g.N = static_cast<int>(N); g.C = static_cast<int>(C);
   g.rowptr = rowptr; g.src = src;
   g.aggr = DGCN_AGGR_ADD; g.raw = 1;
   g.out = out;
@@ -137,8 +121,14 @@ int dgcn_gin_sage_aggregate(int32_t rule, const float* x, int64_t N, int64_t C, 
     g.hub_row_count = hubs->counts + 1; g.hub_min_degree = hubs->min_degree; g.hub_seg_edges = hubs->seg_edges;
     g.hub_partial = hubs->partial;
   }
-  const bool vec4 = (C % 4) == 0 && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out)) & 15) == 0;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (dtype != DGCN_F32) {   // half rows: 8-byte row loads (4 channels per lane), fp32 out stored as float4
+    if ((C % 4) != 0 || C > 1024 || (reinterpret_cast<uintptr_t>(x) & 7) != 0 ||
+        (reinterpret_cast<uintptr_t>(out) & 15) != 0)
+      return DGCN_ERR_UNSUPPORTED;
+    return launch_gin_sage_half(g, dtype, rule == DGCN_GIN, s);
+  }
+  const bool vec4 = (C % 4) == 0 && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out)) & 15) == 0;
   return rule == DGCN_GIN ? dispatch_gin_sage<RULE_GIN>(g, vec4, s) : dispatch_gin_sage<RULE_SELF_LOOP>(g, vec4, s);
 }
 

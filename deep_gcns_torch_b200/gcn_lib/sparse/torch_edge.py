@@ -28,10 +28,14 @@ def _clouds(x, batch):
 
 
 def _knn_flat(x, k, dilation, cols, batch):
-    """(N_total, C) -> (nn_idx, center_idx), each (1, N_total*k) int64 with global point numbers."""
+    """(N_total, C) -> (nn_idx, center_idx), each (1, N_total*k) int64 with global point numbers.  bf16 / fp16
+    features (torch.autocast) are widened to fp32 in the transposed copy the selection kernels read anyway, so the
+    graph is the one of x.float()."""
     with torch.no_grad():
         B, n = _clouds(x, batch)
-        xb = x.detach().reshape(B, n, x.shape[-1]).transpose(1, 2).contiguous().unsqueeze(-1)   # (B,C,n,1)
+        dtype = torch.float32 if x.dtype in (torch.bfloat16, torch.float16) else x.dtype
+        xb = x.detach().reshape(B, n, x.shape[-1]).transpose(1, 2).to(dtype, memory_format=torch.contiguous_format)
+        xb = xb.unsqueeze(-1)                                                                     # (B,C,n,1)
         ei, _ = _native.knn_graph(xb, k, dilation, cols=cols)                                   # (2,B,n,k) local ids
         start = torch.arange(0, B * n, n, device=x.device).view(1, B, 1, 1)
         ei = ei + start

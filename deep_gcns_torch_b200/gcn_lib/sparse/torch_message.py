@@ -90,17 +90,18 @@ class _AggregateFn(torch.autograd.Function):
 
 class _GinSageFn(torch.autograd.Function):
     """GIN's sum_j x_j + (1 + eps) x_i, or GraphSAGE's mean over {j -> i, j != i} + {i} of x_j ('sage') / x_j - x_i
-    ('rsage'), over the cached CSR graph; see dgcn_gin_sage_aggregate.  eps: GIN's (1,) buffer (no gradient) or None."""
+    ('rsage'), over the cached CSR graph; see dgcn_gin_sage_aggregate.  eps: GIN's (1,) buffer (no gradient) or None.
+    The output is fp32 for fp32, bf16 and fp16 x; the gradient is returned in x's dtype."""
 
     @staticmethod
     def forward(ctx, rule, csr, x, eps):
-        ctx.rule, ctx.csr, ctx.eps = rule, csr, eps
+        ctx.rule, ctx.csr, ctx.eps, ctx.x_dtype = rule, csr, eps, x.dtype
         return _native.gin_sage_aggregate(rule, x, csr, eps)
 
     @staticmethod
     def backward(ctx, grad_out):
-        gx = _native.gin_sage_aggregate_backward(ctx.rule, grad_out, ctx.csr, ctx.eps) if ctx.needs_input_grad[2] \
-            else None
+        gx = _native.gin_sage_aggregate_backward(ctx.rule, grad_out, ctx.csr, ctx.eps).to(ctx.x_dtype) \
+            if ctx.needs_input_grad[2] else None
         return None, None, gx, None
 
 

@@ -167,10 +167,11 @@ class EdgConv(BasicConvLowering, nn.Module):
                                  None if bn is None else bn.weight, None if bn is None else bn.bias)
 
 
-def _fp32_cuda_input(layer, x, edge_index):
+def _cuda_rows_input(layer, x, edge_index):
+    """GIN / GraphSAGE node features: fp32, or bf16 / fp16 (torch.autocast), which the aggregate reads as they are."""
     _native._require_cuda(x, edge_index)
-    if x.dtype != torch.float32:
-        raise RuntimeError("%s computes in fp32, got %s features" % (layer, x.dtype))
+    if x.dtype not in _native._ROW_DTYPE:
+        raise RuntimeError("%s takes fp32, bf16 or fp16 features, got %s" % (layer, x.dtype))
 
 
 class GinConv(nn.Module):
@@ -181,7 +182,8 @@ class GinConv(nn.Module):
     torch_geometric's: the sum first, then + (1 + eps) * x (one rounding for the product, one for the add).  The
     aggregation is one pass of the CSR kernel over the cached graph (dgcn_gin_sage_aggregate, forward and backward);
     the MLP stays torch, so a BatchNorm in it may be an nn.SyncBatchNorm.  `aggr` is accepted and unused, as in the
-    reference.  fp32 CUDA tensors only."""
+    reference.  CUDA tensors, fp32 or bf16 / fp16 features: half rows give the bits of their fp32 upcast and their
+    gradient comes back in their own dtype (the fp32 gradient rounded once)."""
 
     def __init__(self, in_channels, out_channels, act="relu", norm=None, bias=True, aggr="add"):
         super().__init__()
@@ -190,7 +192,7 @@ class GinConv(nn.Module):
         self.nn = MLP([in_channels, out_channels], act, norm, bias)
 
     def forward(self, x, edge_index):
-        _fp32_cuda_input("GinConv", x, edge_index)
+        _cuda_rows_input("GinConv", x, edge_index)
         csr = csr_of(edge_index, x.size(0))
         return self.nn(_GinSageFn.apply("gin", csr, x, self.eps))
 
@@ -206,7 +208,8 @@ class SAGEConv(nn.Module):
     The message is linear, so the mean runs on the raw rows in the CSR kernel over the cached graph
     (dgcn_gin_sage_aggregate: (sum_{j != i} x_j + x_i) / c_i, relative (sum_{j != i} x_j - (c_i - 1) x_i) / c_i,
     equal to the reference up to re-association) and W, nn, bias and the normalisation stay torch.  With `size`,
-    the mean over edge_index as given (an empty row gives 0).  fp32 CUDA tensors only."""
+    the mean over edge_index as given (an empty row gives 0).  CUDA tensors, fp32 or bf16 / fp16 features, as in
+    GinConv."""
 
     def __init__(self, in_channels, out_channels, nn, norm=True, bias=True, relative=False, **kwargs):
         super().__init__()
@@ -229,7 +232,7 @@ class SAGEConv(nn.Module):
 
     def forward(self, x, edge_index, size=None):
         x = x.unsqueeze(-1) if x.dim() == 1 else x
-        _fp32_cuda_input(type(self).__name__, x, edge_index)
+        _cuda_rows_input(type(self).__name__, x, edge_index)
         if size is None:
             csr = csr_of(edge_index, x.size(0))
             aggr = _GinSageFn.apply("rsage" if self.relative else "sage", csr, x, None)

@@ -387,19 +387,21 @@ int dgcn_res_plus_backward_dh(const float* g_y, const float* h, int64_t N, int64
  *               edges j -> i with j != i) + 1, out_i = (sum_{j->i, j != i} x_j + x_i) / c_i;
  *   DGCN_RSAGE: the same set with messages x_j - x_i (the added loop's message is 0):
  *               out_i = (sum_{j->i, j != i} x_j - (c_i - 1) * x_i) / c_i.
- * x (N, C) fp32 row-major, out (N, C) fp32, C <= 1024 (float4 lanes when C % 4 == 0 and x, out are 16-byte
- * aligned, one channel per lane otherwise, with the same result); C > 1024 returns DGCN_ERR_UNSUPPORTED.  hubs:
- * dgcn_csr_hubs or NULL (rows of in-degree >= min_degree are then aggregated in segments, with the same result up to
- * fp32 re-association). */
+ * x (N, C) row-major of element type dtype (dgcn_dtype), out (N, C) fp32, C <= 1024; C > 1024 returns
+ * DGCN_ERR_UNSUPPORTED.  fp32 rows: float4 lanes when C % 4 == 0 and x, out are 16-byte aligned, one channel per lane
+ * otherwise, with the same result.  DGCN_BF16 / DGCN_F16 rows are widened exactly in registers and the result is
+ * bit-identical to the fp32 call on the same rows converted to fp32; they need C % 4 == 0, an 8-byte aligned x and a
+ * 16-byte aligned out, and anything else returns DGCN_ERR_UNSUPPORTED.  hubs: dgcn_csr_hubs or NULL (rows of
+ * in-degree >= min_degree are then aggregated in segments, with the same result up to fp32 re-association). */
 enum dgcn_gin_sage { DGCN_GIN = 0, DGCN_SAGE = 1, DGCN_RSAGE = 2 };
-int dgcn_gin_sage_aggregate(int32_t rule, const float* x, int64_t N, int64_t C, const int32_t* rowptr,
+int dgcn_gin_sage_aggregate(int32_t dtype, int32_t rule, const void* x, int64_t N, int64_t C, const int32_t* rowptr,
                             const int32_t* src, const dgcn_csr_hubs* hubs /* may be NULL */, const float* eps,
                             float* out, dgcn_stream_t stream);
 /* Gradient of dgcn_gin_sage_aggregate w.r.t. x: grad_x (N, C) must be zero-initialised by the caller (rows are
  * accumulated with atomics, so the order of the additions - and the last bits - varies from run to run).  Every
  * source of an edge j -> i receives grad_out_i (GIN) or grad_out_i / c_i (SAGE, RSAGE; edges with j != i only); row i
  * receives (1 + eps) * grad_out_i (GIN), grad_out_i / c_i (SAGE) or -(c_i - 1) / c_i * grad_out_i (RSAGE).
- * C <= 1024. */
+ * x is not read, so the same call serves fp32 and half rows (the caller rounds grad_x to x's type).  C <= 1024. */
 int dgcn_gin_sage_aggregate_backward(int32_t rule, int64_t N, int64_t C, const int32_t* rowptr, const int32_t* src,
                                      const float* eps, const float* grad_out, float* grad_x, dgcn_stream_t stream);
 

@@ -237,7 +237,7 @@ def _check(rc, what):
         msg = l.dgcn_status_string(rc).decode()
         extra = l.dgcn_last_cuda_error().decode() if rc == -4 else ""
         # DGCN_ERR_UNSUPPORTED: a valid request the kernels do not cover (NotImplementedError is a RuntimeError)
-        raise (NotImplementedError if rc == -2 else RuntimeError)("%s failed: %s %s" % (what, msg, extra))
+        raise (NotImplementedError if rc == ERR_UNSUPPORTED else RuntimeError)("%s failed: %s %s" % (what, msg, extra))
 
 
 def _ptr(t):
@@ -613,6 +613,36 @@ def _keep_mask(keep):
     return KeepMaskC(_ptr(bits), bits.shape[1], float(keep[1])), bits
 
 
+ERR_UNSUPPORTED = -2       # dgcn_status: a valid request the kernels do not cover
+RAW_MAX_C = 1024           # raw aggregate, forward: the widest launch on float4 rows (C % 4 == 0, 16-byte aligned) ...
+RAW_MAX_C_VEC1 = 256       # ... and on any other rows (one channel per lane)
+RAW_MAX_C_BWD = 512        # ... backward: the widest launch
+
+
+def raw_channel_slices(C, backward=False):
+    """[(c0, c1)]: contiguous channel slices covering 0 .. C, each a launch the raw aggregate kernels accept on a fresh
+    contiguous (so 16-byte aligned) copy of its rows.  Backward: RAW_MAX_C_BWD channels at a time.  Forward: RAW_MAX_C
+    at a time, and a last slice that is wider than RAW_MAX_C_VEC1 with C % 4 != 0 becomes its multiple-of-4 part plus
+    the last C % 4 channels."""
+    step = RAW_MAX_C_BWD if backward else RAW_MAX_C
+    cuts = list(range(0, C, step)) + [C]
+    if not backward and C % 4 and C - cuts[-2] > RAW_MAX_C_VEC1:
+        cuts.insert(-1, C - C % 4)
+    return list(zip(cuts[:-1], cuts[1:]))
+
+
+def _fresh(t):
+    """A contiguous copy of t in a new (so 16-byte aligned) allocation, even when t is contiguous already."""
+    return t.clone(memory_format=torch.contiguous_format)
+
+
+def _channel_separable(prm, x_dst, edge_attr, pre, keep, rows=None, skip_hubs=False):
+    """Raw messages without MsgNorm, residual, edge rows or block fusion: every output channel depends on its own input
+    channel only, so the aggregate may run on channel slices.  (MsgNorm couples the channels of a row.)"""
+    return bool(prm.raw_message) and not prm.msg_norm and not prm.add_residual and x_dst is None and \
+        edge_attr is None and pre is None and keep is None and rows is None and not skip_hubs
+
+
 def genconv_aggregate(x_src, x_dst, csr, prm, edge_attr=None, out=None, pre=None, rows=None, skip_hubs=False,
                       keep=None):
     """dgcn_genconv_aggregate: out (N, C) = x_dst + MsgNorm(aggregate(message)).
@@ -621,7 +651,26 @@ def genconv_aggregate(x_src, x_dst, csr, prm, edge_attr=None, out=None, pre=None
     pre = (scale (C), shift (C), relu): rows of x_src / x_dst are read as act(scale * x + shift).
     keep = (bits, keep_scale) (dgcn_keep_mask, with pre and relu): rows are read as
     keep ? relu(scale * x + shift) * keep_scale : 0 (dropout in training).
-    rows (int32) / skip_hubs: destination rows of this launch (dgcn_genconv_fusion)."""
+    rows (int32) / skip_hubs: destination rows of this launch (dgcn_genconv_fusion).
+    Raw messages (prm.raw_message, x_dst None, nothing fused) at a C the kernels refuse - C > RAW_MAX_C, or
+    C > RAW_MAX_C_VEC1 on rows that are not float4-able - run as one launch per raw_channel_slices slice, each on a
+    contiguous copy of its channels, written into one (N, C) output.  Each channel sums or compares the same edges in
+    the same order in any channel block, so the bits are those a single launch would give."""
+    rc, out = _genconv_aggregate(x_src, x_dst, csr, prm, edge_attr, out, pre, rows, skip_hubs, keep)
+    if rc == ERR_UNSUPPORTED and _channel_separable(prm, x_dst, edge_attr, pre, keep, rows, skip_hubs):
+        x_src = x_src.detach()
+        for c0, c1 in raw_channel_slices(x_src.shape[1]):
+            rc, part = _genconv_aggregate(_fresh(x_src[:, c0:c1]), None, csr, prm)
+            _check(rc, "dgcn_genconv_aggregate")
+            out[:, c0:c1] = part
+        return out
+    _check(rc, "dgcn_genconv_aggregate")
+    return out
+
+
+def _genconv_aggregate(x_src, x_dst, csr, prm, edge_attr=None, out=None, pre=None, rows=None, skip_hubs=False,
+                       keep=None):
+    """One dgcn_genconv_aggregate call: (status, out)."""
     rowptr, src, eid = csr[:3]
     _require_cuda(x_src, x_dst, rowptr, src, eid, edge_attr, out, rows, None if keep is None else keep[0])
     dtype, x_src, x_dst, edge_attr = aggregate_rows(x_src, x_dst, edge_attr, pre=pre)
@@ -652,21 +701,41 @@ def genconv_aggregate(x_src, x_dst, csr, prm, edge_attr=None, out=None, pre=None
                     raise RuntimeError("genconv_aggregate: rows must be a contiguous int32 tensor")
                 fus.row_list, fus.n_rows = (rows.data_ptr() or None), rows.numel()
                 if rows.numel() == 0 and skip_hubs:
-                    return out
+                    return 0, out
         rc = lib().dgcn_genconv_aggregate(dtype, _ptr(x_src), _ptr(x_dst), N, C, _ptr(rowptr), _ptr(src), _ptr(eid),
                                           _ptr(edge_attr), ctypes.byref(prm),
                                           ctypes.byref(hubs) if hubs is not None else None,
                                           ctypes.byref(fus) if fus is not None else None,
                                           ctypes.byref(km) if km is not None else None, _ptr(out), _stream(dev))
-        _check(rc, "dgcn_genconv_aggregate")
-    return out
+    return rc, out
 
 
 def genconv_aggregate_backward(x_src, x_dst, csr, prm, grad_out, edge_attr=None, softmax_grad=False,
                                need_edge_attr=False, pre=None, keep=None):
     """dgcn_genconv_aggregate_backward: (grad_x_src (N_src,C) fp32, grad_x_dst (N,C) fp32 | None,
     grad_edge_attr in edge_attr's row dtype | None, grad_scalars (4) = d/dt, d/dp, d/dy, d/dmsg_scale).
-    pre / keep: the forward's (genconv_aggregate); the row gradients are then w.r.t. the activated rows."""
+    pre / keep: the forward's (genconv_aggregate); the row gradients are then w.r.t. the activated rows.
+    Raw messages past RAW_MAX_C_BWD channels (x_dst None, nothing fused) run as one launch per raw_channel_slices
+    slice, as in genconv_aggregate; the scalar gradients are summed over the slices."""
+    rc, res = _genconv_aggregate_backward(x_src, x_dst, csr, prm, grad_out, edge_attr, softmax_grad, need_edge_attr,
+                                          pre, keep)
+    if rc == ERR_UNSUPPORTED and _channel_separable(prm, x_dst, edge_attr, pre, keep):
+        gsrc, gsc = res[0], res[3]
+        x_src, grad_out = x_src.detach(), grad_out.detach()
+        for c0, c1 in raw_channel_slices(x_src.shape[1], backward=True):
+            rc, part = _genconv_aggregate_backward(_fresh(x_src[:, c0:c1]), None, csr, prm,
+                                                   _fresh(grad_out[:, c0:c1]), softmax_grad=softmax_grad)
+            _check(rc, "dgcn_genconv_aggregate_backward")
+            gsrc[:, c0:c1] = part[0]
+            gsc += part[3]
+        return res
+    _check(rc, "dgcn_genconv_aggregate_backward")
+    return res
+
+
+def _genconv_aggregate_backward(x_src, x_dst, csr, prm, grad_out, edge_attr=None, softmax_grad=False,
+                                need_edge_attr=False, pre=None, keep=None):
+    """One dgcn_genconv_aggregate_backward call: (status, (grad_x_src, grad_x_dst, grad_edge_attr, grad_scalars))."""
     rowptr, src, eid = csr[:3]
     _require_cuda(x_src, x_dst, grad_out, edge_attr)
     dtype, x_src, x_dst, edge_attr = aggregate_rows(x_src, x_dst, edge_attr, pre=pre, backward=True)
@@ -693,8 +762,7 @@ def genconv_aggregate_backward(x_src, x_dst, csr, prm, grad_out, edge_attr=None,
                                                    int(bool(pre[2])) if pre is not None else 0,
                                                    ctypes.byref(km) if km is not None else None, _ptr(grad_out),
                                                    _ptr(gsrc), _ptr(gdst), _ptr(gea), _ptr(gsc), _stream(dev))
-        _check(rc, "dgcn_genconv_aggregate_backward")
-    return gsrc, gdst, gea, gsc
+    return rc, (gsrc, gdst, gea, gsc)
 
 
 def _gin_sage_args(rule, x, csr, eps, half_rows=False):

@@ -85,7 +85,8 @@ class MRConv(nn.Module):
     nn(cat[x, scatter_(aggr, x_j - x_i, dst)]).  x_i is constant over a destination's edges and fp32 subtraction
     is monotone, so max_j fl(x_j - x_i) = fl(max_j x_j - x_i) bit for bit: the aggregation runs on the raw source
     rows in the CSR kernel and x_i is subtracted once per node ('add' / 'mean': sum_j x_j - deg * x_i, equal up to
-    re-association)."""
+    re-association).  Any C: past the kernels' widest launch the aggregation runs on channel slices (raw messages
+    are channel-separable), with the bits of one launch."""
 
     def __init__(self, in_channels, out_channels, act="relu", norm=None, bias=True, aggr="max"):
         super().__init__()
@@ -100,9 +101,11 @@ class MRConv(nn.Module):
             m = -m
         else:
             m, csr = _aggregate_rows(self.aggr, x, edge_index)
-        deg = (csr[0][1:] - csr[0][:-1]).to(x.dtype).unsqueeze(1)
+        deg = (csr[0][1:] - csr[0][:-1]).unsqueeze(1)
         if self.aggr == "add":
-            x_j = m - deg * x
+            # deg * x_i in fp32 (at least): in bf16 / fp16 the product of a hub row's degree keeps 8 / 11 bits, and
+            # the subtraction from the fp32 sum m cancels most of it
+            x_j = m - deg.to(torch.promote_types(x.dtype, torch.float32)) * x
         else:
             x_j = torch.where(deg > 0, m - x, torch.zeros_like(m))
         return self.nn(torch.cat([x, x_j], dim=1))
